@@ -1,18 +1,20 @@
 #!/usr/bin/env python3
-"""bench.py -- rows scanned/s of the LogsQL block-scan hot path on B200 (BASELINE.json metric), one process per GPU.
+"""bench.py -- rows scanned/s of the LogsQL block-scan hot path on H100 (BASELINE.json metric), one process per GPU.
 
     python bench.py [--gpus N] [--steps K] [--warmup W]            # GPU arm (libvlscan.so)
     python bench.py --impl reference [--gpus N] [--steps K] ...    # reference arm: the CPU algorithm on the host cores
+    python bench.py ... --dump-outputs DIR                         # also write the timed scan's last result as DIR/*.npy
 
 A "step" is one pass of the hot path over one batch of synthetic blocks:  bm.init/setBits + filter.applyToBlockSearch for every
 block (lib/logstorage/block_search.go:207-215).
 
-Workload at N=1: BASELINE.json configs[2] (C3, the config the north-star target is quoted on and the largest one that fits one GPU):
-`_msg:~"conn.*refused"` over 1 B vlogsgenerator-shaped rows, 32 fields => 2000 rows/block by the 2 MB rule, 500 000 blocks, ~142 GB
-of `_msg` bytes + lens items + bloom filters resident in HBM when the timed region starts (`value`).  `e2e` is the same filter through
+Workload at N=1: BASELINE.json configs[2] (C3, the config the north-star target is quoted on):
+`_msg:~"conn.*refused"` over 400 M vlogsgenerator-shaped rows, 32 fields => 2000 rows/block by the 2 MB rule, 200 000 blocks, ~57 GB
+of `_msg` bytes + lens items + bloom filters resident in HBM when the timed region starts (`value`); 1 B rows (~142 GB) do not fit
+the 80 GB of one H100.  `e2e` is the same filter through
 the C-ABI call vlscan_scan_batch on pinned HOST buffers holding the blocks in their on-disk form (ZSTD frames), H2D + device decode +
 scan + D2H inside the timed region, on the first --e2e-rows rows of the same data set per step (a search worker hands the part over
-batch by batch; host staging of all 1e9 rows would need ~60 GB of pinned memory and minutes of writer-side compression).
+batch by batch; host staging of all 4e8 rows would need ~24 GB of pinned memory and minutes of writer-side compression).
 C2 and C4 (BASELINE.json configs[1], configs[3]) are measured in the same run and reported under `extra_workloads`.
 
 Parity inside the bench: the first --cpu-sample-rows rows of the benched batch are also scanned by the CPU oracle; the digest of its
@@ -45,7 +47,7 @@ WORKLOADS = {
     "C1": dict(rows=1_000_000, fields=8, rows_per_block=6400, mask=0b0001, logsql='_msg:"error"', tree=lambda F: F.phrase("_msg", "error")),
     "C2": dict(rows=100_000_000, fields=16, rows_per_block=3000, mask=0b0011, logsql='_msg:"timeout" AND level:error',
                tree=lambda F: F.and_([F.phrase("_msg", "timeout"), F.phrase("level", "error")])),
-    "C3": dict(rows=1_000_000_000, fields=32, rows_per_block=2000, mask=0b0001, logsql='_msg:~"conn.*refused"', tree=lambda F: F.regexp("_msg", "conn.*refused")),
+    "C3": dict(rows=400_000_000, fields=32, rows_per_block=2000, mask=0b0001, logsql='_msg:~"conn.*refused"', tree=lambda F: F.regexp("_msg", "conn.*refused")),
     "C4": dict(rows=125_000_000, fields=32, rows_per_block=2000, mask=0b1101, logsql='_msg:"GET" AND path:api* AND status:in(500,502,503)',
                tree=lambda F: F.and_([F.phrase("_msg", "GET"), F.prefix("path", "api"), F.in_("status", ["500", "502", "503"])])),
 }
@@ -70,11 +72,13 @@ def parse_args():
     ap.add_argument("--cpu-sample-rows", type=int, default=12_000_000)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the extra workloads (C2, C4) measured next to the headline at N=1")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the result of the last timed scan (rank 0) as DIR/<name>.npy for output-by-output comparison of builds")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -114,7 +118,7 @@ def hbm_peak():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(peaks["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet 3.35 TB/s (not a measured peak)"
 
 
 def ncu_traffic(workload, rows):
@@ -195,15 +199,12 @@ def run_reference(args, wl, gen_kw, rank, world):
     if rank != 0:
         return
     threads = os.cpu_count() or 1
-    t0 = time.time()
     rates, info = [], None
-    n = args.warmup + max(args.steps, 5)
+    n = args.warmup + args.steps
     for i in range(n):
         rate, info = cpu_port(wl, gen_kw, args.cpu_sample_rows, threads, target_secs=min(8.0, 160.0 / n))
         if i >= args.warmup:
             rates.append(rate)
-        if time.time() - t0 > 200 and len(rates) >= 3:
-            break
     value = statistics.median(rates)
     hi = host_info()
     out = {
@@ -228,6 +229,29 @@ def words_digest(vloracle, words, rows_list, key_base):
         d ^= (vloracle.xxh64(words[off:off + nw].tobytes()) * (2 * (key_base + i) + 1)) & 0xFFFFFFFFFFFFFFFF
         off += nw
     return d
+
+
+DUMP_SAMPLE_ROWS = 1 << 21
+
+
+def dump_outputs(out_dir, words, counts, rows, rows_per_block):
+    """What a caller of the timed path receives - the row bitmap and the match count of every block - as float .npy files (~25 MB + 8 B
+    per block):
+    block_match_counts (every block), row_match_sample (0/1 of a fixed seeded sample of rows, all rows when there are fewer) and
+    row_match_sample_index (the sampled row numbers).  Blocks hold rows_per_block rows each except the last, so row r sits in word
+    (r // rows_per_block) * words_per_block + (r % rows_per_block) // 64."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    if rows <= DUMP_SAMPLE_ROWS:
+        idx = np.arange(rows, dtype=np.int64)
+    else:
+        idx = np.unique(np.random.default_rng(SEED).integers(0, rows, size=DUMP_SAMPLE_ROWS, dtype=np.int64))
+    wpb = (rows_per_block + 63) // 64
+    blk, pos = idx // rows_per_block, idx % rows_per_block
+    bits = (words[blk * wpb + pos // 64] >> (pos % 64).astype(np.uint64)) & np.uint64(1)
+    np.save(os.path.join(out_dir, "block_match_counts.npy"), counts.astype(np.float64))
+    np.save(os.path.join(out_dir, "row_match_sample.npy"), bits.astype(np.float32))
+    np.save(os.path.join(out_dir, "row_match_sample_index.npy"), idx.astype(np.float64))
 
 
 def main():
@@ -276,8 +300,9 @@ def main():
         torch.cuda.synchronize()
         ctx.sync()
 
-    def measure(w, w_rows, w_nb, w_kw, steps, warmup, sample_clocks):
-        """resident scan of one workload -> dict; the batch stays alive in the returned dict until the caller frees it"""
+    def measure(w, w_rows, w_nb, w_kw, steps, warmup, sample_clocks, keep_result=False):
+        """resident scan of one workload -> dict; the batch stays alive in the returned dict until the caller frees it.
+        keep_result: also return the bitmap words and per-block match counts of the last timed step (fetched after the timed region)"""
         gcfg = vs.GenConfig(**w_kw)
         block_lo = rank * w_nb
         t_gen = time.time()
@@ -311,6 +336,7 @@ def main():
                 shard.reduce_counters(acc)     # the only collective of the path: ONE final NCCL reduce of the match counters
         ev1.record(stream)
         sync_all()
+        result = ctx.fetch(batch) if keep_result and steps > 0 else None
         clocks = None
         if sampler:
             # the timed region may be shorter than a few nvidia-smi sampling periods: keep the same load running (untimed) until the sampler
@@ -339,7 +365,7 @@ def main():
         step_bytes = st.values_bytes + st.bloom_probe_bytes + st.bitmap_bytes
         return dict(batch=batch, prog=prog, gcfg=gcfg, block_lo=block_lo, ms=ms, steps=steps, st=st, clocks=clocks, t_gen=t_gen, k_avg=k_avg, kbytes=kbytes, achieved=achieved,
                     step_bytes=step_bytes, share=(k_avg / statistics.mean(gms)) if gms and statistics.mean(gms) > 0 else None,
-                    totals=acc.cpu().tolist() if world > 1 else None)
+                    totals=acc.cpu().tolist() if world > 1 else None, result=result)
 
     # ---- the headline workload, resident -----------------------------------------------------------------------------------------
     fallback_note = None
@@ -347,7 +373,7 @@ def main():
     want_rows = rows
     for attempt in range(4):
         try:
-            m = measure(wl, rows, nb, gen_kw, args.steps, args.warmup, True)
+            m = measure(wl, rows, nb, gen_kw, args.steps, args.warmup, True, keep_result=bool(args.dump_outputs) and rank == 0)
             break
         except vs.VlscanError as e:   # does not fit this GPU next to whatever else lives on it: fall back to the largest row count that does
             if "memory" not in str(e).lower() or attempt == 3:
@@ -357,6 +383,8 @@ def main():
     st, batch, prog = m["st"], m["batch"], m["prog"]
     device_bytes = batch.device_bytes
     _, resident_counts = ctx.fetch(batch, bitmaps=False, counts=True)
+    if m["result"] is not None:
+        dump_outputs(args.dump_outputs, *m["result"], rows, wl["rows_per_block"])
 
     # ---- parity of the benched scan against the CPU oracle on its first blocks (device digest vs oracle digest) + CPU baselines ----
     cpu, cpu_post, parity = None, None, None
@@ -433,14 +461,14 @@ def main():
     # ---- the other single-GPU configs of BASELINE.json, same run -------------------------------------------------------------------------
     extra = {}
     if not args.no_extra:
-        # N > 1: C4 is BASELINE.json configs[3] - "1B rows block-sharded 8xB200" is 125 M rows per GPU, so at N = 8 this IS that configuration
+        # N > 1: C4 is BASELINE.json configs[3] - "1B rows block-sharded over 8 GPUs" is 125 M rows per GPU, so at N = 8 this IS that configuration
         for name in (("C2", "C4") if world == 1 else ("C4",)):
             if name == args.workload:
                 continue
             try:
                 w = WORKLOADS[name]
                 w_rows, w_nb, w_kw = gen_args(w, w["rows"])
-                x = measure(w, w_rows, w_nb, w_kw, 10, 3, False)
+                x = measure(w, w_rows, w_nb, w_kw, args.steps, args.warmup, False)
                 extra[name] = {"workload": "%s: %s over %d rows/GPU x %d GPU(s), %d fields" % (name, w["logsql"], w_rows, world, w["fields"]), "value": w_rows * world * x["steps"] / (x["ms"] / 1e3), "unit": "rows/s",
                                "ms_per_step": x["ms"] / x["steps"], "rows_matched": int(x["st"].rows_matched), "gpu_launches_per_step": int(x["st"].gpu_launches),
                                "step_hbm_gbs_per_gpu": (x["step_bytes"] / 1e9) / (x["ms"] / x["steps"] / 1e3),
@@ -497,7 +525,7 @@ def main():
             "data": "synthetic (deterministic vlogsgenerator-shaped rows generated on the device, seed %d)" % SEED,
             "config": {"workload": "%s: %s over %d rows/GPU, %d fields" % (args.workload, wl["logsql"], rows, wl["fields"]), "rows_per_gpu": rows, "rows_per_block": wl["rows_per_block"],
                        "blocks_per_gpu": nb, "hot_block_permille": args.hot_block_permille, "hit_row_permille": args.hit_row_permille,
-                       "l2": "inputs (%.1f GB/GPU) are far larger than the 126 MB L2; no flush between iterations" % (device_bytes / 1e9),
+                       "l2": "inputs (%.1f GB/GPU) are far larger than the 50 MB L2; no flush between iterations" % (device_bytes / 1e9),
                        "parallelism": "blocks sharded over %d GPU(s); counters summed on the device every step, ONE NCCL all-reduce after the last step (inside the timed region)" % world if world > 1 else "1 GPU",
                        "gen_seconds": round(m["t_gen"], 2)},
             "rows_matched_per_gpu": int(st.rows_matched), "blocks_matched_per_gpu": int(st.blocks_matched),
@@ -508,7 +536,7 @@ def main():
             "clocks": m["clocks"],
             "roofline": {"bound": "hbm", "kernel": "k_substr_scan", "achieved": m["achieved"], "peak": peak, "unit": "GB/s", "frac": m["achieved"] / peak if peak else None,
                          "traffic": tr["dram_bytes_per_launch"] if tr else None,
-                         "traffic_source": (tr.get("source") if tr else "no ncu --set full capture of this exact launch size under profiles/ (profiles/ncu_traffic_r02.json lists the ones that exist)"),
+                         "traffic_source": (tr.get("source") if tr else "no ncu --set full capture of this exact launch size recorded (tools/ncu_summary.py --traffic writes profiles/ncu_traffic_r02.json)"),
                          "peak_source": peak_src, "kernel_ms_per_launch": m["k_avg"], "algorithmic_bytes_per_launch": int(m["kbytes"]),
                          "kernel_share_of_step": m["share"]},
             "parity": parity, "e2e": e2e, "cpu_baseline": cpu, "cpu_baseline_post_zstd": cpu_post, "extra_workloads": extra or None, "e2e_bloom_first_staging": bloom_first,

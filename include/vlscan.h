@@ -1,5 +1,5 @@
 /*
- * vlscan.h -- C ABI of the B200-native LogsQL block-scan / filter engine (libvlscan.so).
+ * vlscan.h -- C ABI of the H100-native LogsQL block-scan / filter engine (libvlscan.so).
  *
  * Drop-in boundary for lib/logstorage's query hot path.  The reference has no FFI seam; it is cut at the body of the
  * search-worker loop over one blockSearchWorkBatch (lib/logstorage/storage_search.go:1044-1062): a batch of

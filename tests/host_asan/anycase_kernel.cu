@@ -1,4 +1,4 @@
-// Compile-only check (tests/test_host_asan_cpu.py): the predicates of csrc/vl_anycase.cuh build for sm_100a as device code, i.e. the row
+// Compile-only check (tests/test_host_asan_cpu.py): the predicates of csrc/vl_anycase.cuh build for sm_90a as device code, i.e. the row
 // kernels can call them as they are.  One thread per value; not part of libvlscan.so.
 #include "vl_anycase.cuh"
 

@@ -11,10 +11,10 @@ import pytest
 from victorialogs_b200 import scan as vs
 from parity_util import oracle_block_to_desc, field_names_of
 
-# digests of the walk as it was when the device decoder was last verified on a B200 (commit 0858bd1 .. 1f6f4c9: one thread, std::stable_sort).
-# "groups" was re-pinned in round 2 when the launch-group limits became tapered (vl_zstd_job.h: a small first group, large ones, small ones
+# digests of the single-threaded walk (one thread, std::stable_sort) that the device decoder's parity suite was run against.
+# "groups" was re-pinned when the launch-group limits became tapered (vl_zstd_job.h: a small first group, large ones, small ones
 # over the last twelfth of the sequences - 3 groups for this data set; the frame digest, which does not depend on the cut, is unchanged);
-# the device decoder ran its parity suite on a B200 with those limits.
+# the device decoder's parity suite runs with those limits.
 GOLDEN = {
     "small": (296292749011898157, 13177515279369892816, 15039143775152434337, 10484151172081120490),
     "groups": (17384690534920848810, 2494078724288951318, 166322921929518477, 3889144665088860614),

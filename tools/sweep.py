@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""C5 of BASELINE.json: selectivity / block-clustering sweep of the scan on one B200 (resident inputs).
+"""C5 of BASELINE.json: selectivity / block-clustering sweep of the scan on one H100 (resident inputs).
 
 For every (workload, hot_block_permille, hit_row_permille) point: generate the data set on the device, run W warm-up + K timed scans
 (CUDA events on the ctx stream), and report rows/s, ms/step, how many blocks the bloom pre-pass pruned ("bloom-only" blocks: their
@@ -9,7 +9,7 @@ Vocabulary rows all carry the entry the workload's query looks for (`columns_mas
 hit_row_permille x hot_block_permille IS the row selectivity of the leading leaf: the sweep reaches 0.5 and 1.0, not just the 8 % a uniform
 draw over the 12 vocabulary entries allows.
 
-    python tools/sweep.py --rows 100000000 --out profiles/sweep_r02.json
+    python tools/sweep.py --rows 100000000 --out sweep.json
 """
 import argparse
 import json

@@ -1,9 +1,10 @@
 #!/bin/bash
-# Builds libvlscan.so (CUDA kernels + C ABI) for sm_100a. nvcc cross-compiles without a GPU.
+# Builds libvlscan.so (CUDA kernels + C ABI) for sm_90a (H100). nvcc cross-compiles without a GPU.
 set -e
 cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall,-Wno-unused-function -Xcudafe --diag_suppress=177 ${VL_NVCC_EXTRA}"
+ARCH="-gencode arch=compute_90a,code=sm_90a"
+FLAGS="$ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall,-Wno-unused-function -Xcudafe --diag_suppress=177 ${VL_NVCC_EXTRA}"
 mkdir -p build
 pids=()
 for tu in vl_engine vl_gen vl_zstd; do
@@ -11,5 +12,5 @@ for tu in vl_engine vl_gen vl_zstd; do
     pids+=($!)
 done
 for p in "${pids[@]}"; do wait $p; done
-$NVCC -gencode arch=compute_100a,code=sm_100a -shared -o libvlscan.so build/vl_engine.o build/vl_gen.o build/vl_zstd.o -ldl
+$NVCC $ARCH -shared -o libvlscan.so build/vl_engine.o build/vl_gen.o build/vl_zstd.o -ldl
 echo built victorialogs_b200/libvlscan.so

@@ -106,7 +106,7 @@ struct vlscan_ctx {
     vlscan_batch* recycle = nullptr;       // staging batch reused by vlscan_scan_batch
     bool has_result = false;
     uint64_t last_launches = 0;
-    int sm_count = 148;
+    int sm_count = 132;                    // H100 SXM; vlscan_ctx_create reads the device's own count
     int scan_occ[2] = {1, 1};              // resident CTAs per SM of k_substr_scan<false> / <true> on this device
     int row_occ = 1;                       // ... and of k_row_match (its persistent grid is exactly the resident set)
     void* ensure_pinned(size_t n);

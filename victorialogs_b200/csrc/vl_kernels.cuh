@@ -1,4 +1,4 @@
-// CUDA kernels of the block-scan engine (sm_100a).  HBM-bound byte / bitmap work: coalesced 16-byte vector loads,
+// CUDA kernels of the block-scan engine (sm_90a).  HBM-bound byte / bitmap work: coalesced 16-byte vector loads,
 // warp ballots / shuffles, no tensor cores.  Each kernel names the reference code it replaces.
 #pragma once
 #include <cuda_runtime.h>
@@ -817,9 +817,8 @@ static __device__ __forceinline__ uint32_t scan_vector_hit(const uint4& v, const
 // VECTOR) to a queue in shared memory and goes on streaming; out of the queue, the CTA's 256 threads take one vector each, re-read it (it is
 // still in L2), enumerate its candidate words / alignments and verify them.  Verifying in place costs a chain of ~6 dependent memory round trips
 // (column header, row offsets, lens items, neighbouring bytes) during which the other 31 lanes of the warp wait; in the drain all lanes are
-// busy and the chains overlap.  Round 2, second step: the streaming side used to enumerate the candidates itself (4 compares on each of a
-// lane's 16 words, by every lane of a warp in which ANY lane had a hit): at selectivity 0.5 that enumeration was 43 % of all instructions of
-// the kernel (profiles/kernel_history_r02.md).  Now it only ballots which lanes have a hit in each of their four vectors and reserves queue
+// busy and the chains overlap.  The streaming side does not enumerate the candidates itself (4 compares on each of a lane's 16 words, by
+// every lane of a warp in which ANY lane had a hit): at dense selectivities that enumeration dominates the kernel's instructions.  It only ballots which lanes have a hit in each of their four vectors and reserves queue
 // slots with one shared-memory atomic per vector index.  The queue is drained when a tile ends with at least VL_SCAN_QFLUSH entries, and when
 // the CTA has run out of tiles.  A vector that finds the queue full is handled by its lane on the spot.
 #define VL_SCAN_QCAP 2048
@@ -923,7 +922,7 @@ static __device__ __noinline__ void scan_drain(const DevProgram& P, const BatchV
     }
 }
 
-// Persistent grid: 148 SMs x 5 resident CTAs x 256 threads, each CTA strides over the tile table built by k_plan_leaf.  Per round a thread has
+// Persistent grid: SMs (132 on an H100) x 5 resident CTAs x 256 threads, each CTA strides over the tile table built by k_plan_leaf.  Per round a thread has
 // four independent LDG.128 in flight, 16 KiB apart (a warp's requests spread over more L2 slices / HBM channels than adjacent 4 KiB slices would).
 template <bool MASKED>
 static __global__ void __launch_bounds__(VL_SCAN_THREADS, 5) k_substr_scan(const __grid_constant__ DevProgram P, const __grid_constant__ BatchView B, int slot, const __grid_constant__ ScanParams sp, const uint32_t* __restrict__ tile_block,

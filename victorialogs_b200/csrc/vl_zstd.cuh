@@ -15,8 +15,7 @@
 //   k_execute       one warp  per frame                      (literal runs as one flat copy, matches in dependency order)
 //
 // Tables that a later block may reuse (Treeless literals, Repeat_Mode) live in per-block slots in HBM; the host resolves which
-// slot a block reads while it walks the block headers (it needs those for the layout anyway).  DESIGN.md §3.5 has the full picture,
-// profiles/zstd_history_r01.md the measurements behind each choice.
+// slot a block reads while it walks the block headers (it needs those for the layout anyway).  DESIGN.md §3.5 has the full picture.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -410,7 +409,7 @@ static __global__ void __launch_bounds__(64) k_fse_build(ZView V, const uint32_t
 //     with bfe) come out of it with one funnel shift each; the position is a single 32-bit bit index relative to a 256-byte aligned origin;
 //   * errors are sticky bits checked once after the loop; the last sequence (no state update) is peeled off.
 // (Round 2 also tried FOUR lanes per block - one FSE state per lane of a quad, widths exchanged by shuffles, 7 warps per SM: byte-exact, but
-// 67 ms instead of 38 ms on 100 M rows of C2; the shuffles put ~90 instructions on every sequence of every quad.  profiles/zstd_history_r02.md)
+// slower; the shuffles put ~90 instructions on every sequence of every quad.)
 static const uint32_t Z_SEQ_CTA_LANES = 56;
 static const uint32_t Z_LINEBUF = 272;    // bytes of shared memory per lane: the 256-byte ring + a 16-byte skew against bank conflicts
 static const uint32_t Z_SEQ_LEAD = 160;   // the ring is kept filled this many bytes below the reader
@@ -616,7 +615,7 @@ static __global__ void __launch_bounds__(64) k_seq_resolve(ZView V, uint32_t fra
 //   * the next group's sequence records are loaded while the current group is executed.
 // Groups that span the ring or more (a literal run of kilobytes) take the byte-per-lane path of round 1, which also stayed the reference for
 // tests/test_zstd_models_cpu.py.  (Two other round-2 variants were byte-exact but slower: every lane copying its own sequence - a memory
-// wavefront per lane per byte -, and far matches batched beside the literals - they were already in long runs.  profiles/zstd_history_r02.md)
+// wavefront per lane per byte -, and far matches batched beside the literals - they were already in long runs.)
 static const uint32_t Z_RING = 4096;
 static const uint32_t Z_EXEC_WARPS = 4;
 static __device__ __forceinline__ uint32_t ldu32(const uint8_t* p) {   // little-endian 4 bytes at any address: two aligned loads, up to 7 bytes of slack touched

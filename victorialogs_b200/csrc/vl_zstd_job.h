@@ -24,11 +24,11 @@ namespace vl {
 using namespace zs;
 
 // scratch limits of one launch group (groups are cut at frame boundaries)
-// A group must hold enough blocks to fill the device for the lane-per-block phases (148 SMs x 56 sequence lanes = 8.3 k blocks per
-// wave) and enough frames for the warp-per-frame executor (~9 k in flight): small groups decode less efficiently.  On the other hand
+// A group must hold enough blocks to fill the device for the lane-per-block phases (132 SMs x 56 sequence lanes = 7.4 k blocks per
+// wave on an H100) and enough frames for the warp-per-frame executor (~8 k in flight): small groups decode less efficiently.  On the other hand
 // group g is decoded while the bytes of group g+1 are still being copied, so the FIRST group decides when the decoder starts and the LAST
-// one is the tail that nothing hides.  Measured on a B200 (profiles/zstd_history_r02.md): with uniform groups the C3 batch (decode bound)
-// wants the large limits, the C2 batch (DMA bound) half of them.  So the limits are tapered: a small first group, large ones in the middle,
+// one is the tail that nothing hides.  With uniform groups a decode-bound batch (C3) wants the large limits, a DMA-bound one (C2) half
+// of them.  So the limits are tapered: a small first group, large ones in the middle,
 // small ones over the last twelfth of the sequences (walk_values_blocks knows every frame's needs before it cuts).
 // VLSCAN_ZSTD_GROUP_SCALE (tuning only): a fixed multiplier for all groups instead; 4 = the round-1 limits.
 inline uint64_t group_scale_env() { static const uint64_t v = [] { const char* e = getenv("VLSCAN_ZSTD_GROUP_SCALE"); long x = e ? atol(e) : 0; return (uint64_t)(x < 0 ? 0 : x > 64 ? 64 : x); }(); return v; }
