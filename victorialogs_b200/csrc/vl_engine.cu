@@ -583,11 +583,11 @@ struct ScanRun {
         int slot = L.field >= 0 ? field_slot[L.field] : -1;
         uint8_t* action = ctx->action.as<uint8_t>(); uint64_t* payload = ctx->payload.as<uint64_t>(); uint64_t* leaf_bm = ctx->leaf_bm.as<uint64_t>();
         uint32_t* lens_blocks = ctx->lens_blocks.as<uint32_t>(); uint32_t* row_blocks = ctx->row_blocks.as<uint32_t>(); uint32_t* wc = ctx->work_count.as<uint32_t>();
-        uint32_t* tb = ctx->tile_block.as<uint32_t>(); uint32_t* to = ctx->tile_off.as<uint32_t>();
+        ScanTile* tiles = ctx->tiles.as<ScanTile>();
         VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
         if (L.kind == F_EQ_FIELD || L.kind == F_LE_FIELD) {   // two columns, row by row (filter_eq_field.go, filter_le_field.go)
             const int slot_b = field_slot[L.field2];
-            uint32_t* lens_b = tb;   // the tile table is idle for this leaf: it holds the second lens work list
+            uint32_t* lens_b = ctx->lens_blocks2.as<uint32_t>();
             k_plan_pair<<<cdiv((uint64_t)B.nblocks * 32, 256), 256, 0, ctx->stream>>>(P, B, (uint32_t)leaf_idx, slot, slot_b, reg, action, payload, lens_blocks, lens_b, row_blocks, wc, stats);
             launch_check(ctx);
             if (B.nwords) {
@@ -607,7 +607,7 @@ struct ScanRun {
             return;
         }
         // bm.isZero() per block, header dispatch + leaf bloom probe -> per-block action, and the work lists of the kernels below
-        k_plan_leaf<<<cdiv(B.nblocks, VL_PLAN_WARPS), VL_PLAN_WARPS * 32, 0, ctx->stream>>>(P, B, (uint32_t)leaf_idx, slot, reg, action, payload, lens_blocks, row_blocks, tb, to, wc, stats);
+        k_plan_leaf<<<cdiv(B.nblocks, VL_PLAN_WARPS), VL_PLAN_WARPS * 32, 0, ctx->stream>>>(P, B, (uint32_t)leaf_idx, slot, reg, action, payload, lens_blocks, row_blocks, tiles, wc, stats);
         launch_check(ctx);
         if (slot >= 0 && B.nwords) {
             uint32_t* ro = ctx->row_off8[slot].as<uint32_t>(); uint8_t* ready = ctx->ready[slot].as<uint8_t>();
@@ -631,8 +631,8 @@ struct ScanRun {
                 auto& evp = next_scan_events();
                 VL_CUDA(cudaEventRecord(evp.first, ctx->stream));
                 // persistent CTAs: exactly the resident set (SMs x resident CTAs per SM), each striding over the tile table
-                if (masked) k_substr_scan<true><<<ctx->sm_count * ctx->scan_occ[1], VL_SCAN_THREADS, 0, ctx->stream>>>(P, B, slot, sp, tb, to, wc, ro, leaf_bm);
-                else k_substr_scan<false><<<ctx->sm_count * ctx->scan_occ[0], VL_SCAN_THREADS, 0, ctx->stream>>>(P, B, slot, sp, tb, to, wc, ro, leaf_bm);
+                if (masked) k_substr_scan<true><<<ctx->sm_count * ctx->scan_occ[1], VL_SCAN_THREADS, 0, ctx->stream>>>(P, B, slot, sp, tiles, wc, ro, leaf_bm);
+                else k_substr_scan<false><<<ctx->sm_count * ctx->scan_occ[0], VL_SCAN_THREADS, 0, ctx->stream>>>(P, B, slot, sp, tiles, wc, ro, leaf_bm);
                 launch_check(ctx);
                 VL_CUDA(cudaEventRecord(evp.second, ctx->stream));
             }
@@ -663,7 +663,7 @@ struct ScanRun {
             k_plan_pair<<<cdiv((uint64_t)B.nblocks * 32, 256), 256, 0, ctx->stream>>>(P, B, (uint32_t)leaf_idx, slot, field_slot[L.field2], reg, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, stats, need);
         } else {
             if (slot < 0) return;   // a field the batch does not have: nothing to stage
-            k_plan_leaf<<<cdiv(B.nblocks, VL_PLAN_WARPS), VL_PLAN_WARPS * 32, 0, ctx->stream>>>(P, B, (uint32_t)leaf_idx, slot, reg, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, stats, need);
+            k_plan_leaf<<<cdiv(B.nblocks, VL_PLAN_WARPS), VL_PLAN_WARPS * 32, 0, ctx->stream>>>(P, B, (uint32_t)leaf_idx, slot, reg, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, stats, need);
         }
         launch_check(ctx);
     }
@@ -736,10 +736,10 @@ static void do_scan(vlscan_ctx* ctx, const vlscan_program* prog, const vlscan_ba
     for (auto& nd : pr.nodes) run.slots_total += nd.prepass_count;
     uint64_t nb = std::max<uint64_t>(batch->nblocks, 1), nw = std::max<uint64_t>(batch->nwords, 1);
     ctx->action.ensure(nb); ctx->payload.ensure(nb * 8); ctx->leaf_bm.ensure(nw * 8);
-    ctx->lens_blocks.ensure(nb * 4); ctx->row_blocks.ensure(nb * 4); ctx->work_count.ensure(WC_COUNT * 4);
+    ctx->lens_blocks.ensure(nb * 4); ctx->lens_blocks2.ensure(nb * 4); ctx->row_blocks.ensure(nb * 4); ctx->work_count.ensure(WC_COUNT * 4);
     {   // upper bound of 64 KiB tiles of any single column: every payload byte belongs to one column, plus one partial tile per block
         uint64_t max_tiles = batch->arena_bytes / VL_TILE_BYTES + nb + 16;
-        ctx->tile_block.ensure(max_tiles * 4); ctx->tile_off.ensure(max_tiles * 4);
+        ctx->tiles.ensure(max_tiles * sizeof(ScanTile));
     }
     ctx->stats.ensure(ST_COUNT * 8); ctx->totals.ensure(32); ctx->counts.ensure(nb * 4);
     if (ctx->row_off8.size() < batch->nfields) { ctx->row_off8.resize(batch->nfields); ctx->ready.resize(batch->nfields); }
@@ -828,7 +828,7 @@ void vlscan_ctx_free(vlscan_ctx* ctx) {
     cudaSetDevice(ctx->device);
     if (ctx->copy_stream) cudaStreamSynchronize(ctx->copy_stream);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-    for (DevBuf* b : {&ctx->action, &ctx->payload, &ctx->leaf_bm, &ctx->lens_blocks, &ctx->row_blocks, &ctx->work_count, &ctx->stats, &ctx->totals, &ctx->counts, &ctx->slots, &ctx->hit_offs, &ctx->hits, &ctx->tile_block, &ctx->tile_off}) b->release();
+    for (DevBuf* b : {&ctx->action, &ctx->payload, &ctx->leaf_bm, &ctx->lens_blocks, &ctx->row_blocks, &ctx->work_count, &ctx->stats, &ctx->totals, &ctx->counts, &ctx->slots, &ctx->hit_offs, &ctx->hits, &ctx->tiles, &ctx->lens_blocks2}) b->release();
     for (auto& r : ctx->regs) r.release();
     for (auto& r : ctx->row_off8) r.release();
     for (auto& r : ctx->ready) r.release();

@@ -85,7 +85,7 @@ struct vlscan_ctx {
     std::string err;
     uint64_t launches = 0;
     // scratch (grow-only)
-    vl::DevBuf action, payload, leaf_bm, lens_blocks, row_blocks, work_count, stats, totals, counts, slots, hit_offs, hits, tile_block, tile_off;
+    vl::DevBuf action, payload, leaf_bm, lens_blocks, row_blocks, work_count, stats, totals, counts, slots, hit_offs, hits, lens_blocks2, tiles;   // lens_blocks2: second lens work list of a two-column leaf; tiles: ScanTile work list of k_substr_scan
     std::vector<vl::DevBuf> regs;          // bitmap registers of the tree interpreter
     std::vector<vl::DevBuf> row_off8;      // per batch field slot: byte offset of every 8th row (k_lens_offsets)
     std::vector<vl::DevBuf> ready;         // per batch field slot: row_off8 computed for block b in this scan

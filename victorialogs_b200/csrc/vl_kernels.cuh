@@ -264,9 +264,15 @@ static __global__ void k_prepass(DevProgram P, BatchView B, uint32_t pp_begin, u
 #define VL_PLAN_WARPS 8
 enum { WC_LENS = 0, WC_TILES = 1, WC_ROW = 2, WC_LENS2 = 3, WC_COUNT = 4 };   // WC_LENS2: the second column of a two-column leaf
 #define VL_TILE_BYTES 65536u                  /* row bytes per work item of the substring scan */
+// One work item of the substring scan, self-contained so that the streaming side needs one 16-byte load per tile and no column header.
+struct __align__(16) ScanTile {
+    uint64_t off;      // arena byte offset of the tile's first byte
+    uint32_t bytes;    // row bytes in the tile: VL_TILE_BYTES, less for a block's last tile
+    uint32_t block;
+};
 static __global__ void __launch_bounds__(VL_PLAN_WARPS * 32) k_plan_leaf(DevProgram P, BatchView B, uint32_t leaf_idx, int slot, const uint64_t* __restrict__ reg,
                             uint8_t* __restrict__ action, uint64_t* __restrict__ payload, uint32_t* __restrict__ lens_blocks, uint32_t* __restrict__ row_blocks,
-                            uint32_t* __restrict__ tile_block, uint32_t* __restrict__ tile_off, uint32_t* __restrict__ work_count,
+                            ScanTile* __restrict__ tiles, uint32_t* __restrict__ work_count,
                             unsigned long long* __restrict__ stats, uint8_t* __restrict__ need = nullptr) {
     // need != NULL: PROBE pass of a bloom-first upload (phase 1: headers, bloom filters and dict tables are on the device, no values yet).
     // `reg` then only carries which blocks are still alive behind the AND / OR bloom pre-passes of the leaf's ancestors; the kernel runs the
@@ -279,7 +285,7 @@ static __global__ void __launch_bounds__(VL_PLAN_WARPS * 32) k_plan_leaf(DevProg
     const uint32_t b = blockIdx.x * VL_PLAN_WARPS + warp;
     const DevLeaf& L = P.leaves[leaf_idx];
     uint8_t act = ACT_NONE; uint64_t pay = 0;
-    unsigned long long bloom_bytes = 0, values_bytes = 0, scan_bytes = 0; int err = 0;
+    unsigned long long bloom_bytes = 0, values_bytes = 0, scan_bytes = 0, scan_off = 0; int err = 0;
     uint32_t need_lens = 0, need_row = 0, ntiles = 0;
     const bool valid = b < B.nblocks;
     const uint32_t ones = valid ? block_ones_warp(reg, B, b) : 0;
@@ -526,7 +532,7 @@ static __global__ void __launch_bounds__(VL_PLAN_WARPS * 32) k_plan_leaf(DevProg
     }
     if (c && c->kind == COL_VALUES && (act == ACT_SCAN || act >= ACT_ROW)) {
         need_lens = 1;
-        if (act == ACT_SCAN) { ntiles = (uint32_t)((c->data_len + VL_TILE_BYTES - 1) / VL_TILE_BYTES); scan_bytes = c->data_len; }
+        if (act == ACT_SCAN) { ntiles = (uint32_t)((c->data_len + VL_TILE_BYTES - 1) / VL_TILE_BYTES); scan_bytes = c->data_len; scan_off = c->data_off; }
         else need_row = 1;
     }
     }
@@ -552,7 +558,10 @@ static __global__ void __launch_bounds__(VL_PLAN_WARPS * 32) k_plan_leaf(DevProg
     __syncthreads();
     if (need_lens && lane_id() == 0) lens_blocks[s_off[warp][0]] = b;
     if (need_row && lane_id() == 0) row_blocks[s_off[warp][2]] = b;
-    for (uint32_t k = lane_id(); k < ntiles; k += 32) { tile_block[s_off[warp][1] + k] = b; tile_off[s_off[warp][1] + k] = k * VL_TILE_BYTES; }
+    for (uint32_t k = lane_id(); k < ntiles; k += 32) {
+        const uint32_t t0 = k * VL_TILE_BYTES;
+        tiles[s_off[warp][1] + k] = ScanTile{scan_off + t0, (uint32_t)min(scan_bytes - t0, (unsigned long long)VL_TILE_BYTES), b};
+    }
 }
 
 // ---- on-disk columns: header checks of the lens block (unmarshalUint64Items, encoding.go:246-336) once the device has regenerated it ----
@@ -764,10 +773,14 @@ static __device__ __forceinline__ void scan_verify_lane(const DevProgram& P, con
 }
 
 #define VL_SCAN_THREADS 256
-#define VL_SCAN_UNROLL 4                       /* independent 16-byte loads in flight per thread */
+#define VL_SCAN_CTAS 4                         /* resident CTAs per SM the register budget is set for (__launch_bounds__) */
+#define VL_SCAN_UNROLL 4                       /* independent 16-byte loads per thread and round */
 #define VL_SCAN_ROUNDS 4                       /* rounds per tile */
+#define VL_SCAN_STAGES 2                       /* rounds held in registers: STAGES - 1 rounds are in flight while one is evaluated */
+#define VL_SCAN_ROUND_BYTES (VL_SCAN_THREADS * 16)
 #define VL_SCAN_QSTRIDE (VL_TILE_BYTES / VL_SCAN_UNROLL)                          /* distance between a thread's loads of one round */
-static_assert(VL_TILE_BYTES == VL_SCAN_THREADS * 16 * VL_SCAN_UNROLL * VL_SCAN_ROUNDS, "tile size");
+static_assert(VL_TILE_BYTES == VL_SCAN_ROUND_BYTES * VL_SCAN_UNROLL * VL_SCAN_ROUNDS, "tile size");
+static_assert(VL_SCAN_ROUNDS % VL_SCAN_STAGES == 0 && VL_SCAN_STAGES >= 2, "every round of a tile uses the same register stage in every tile");
 
 template <bool MASKED>
 static __device__ __forceinline__ uint32_t scan_word_hits(uint32_t w, const ScanParams& sp) {   // bit r: the word matches pattern r
@@ -823,7 +836,9 @@ static __device__ __forceinline__ uint32_t scan_vector_hit(const uint4& v, const
 // the CTA has run out of tiles.  A vector that finds the queue full is handled by its lane on the spot.
 #define VL_SCAN_QCAP 2048
 #define VL_SCAN_QFLUSH 192
-struct ScanCand { uint32_t block, pos; };   // pos: byte offset of a 16-byte vector inside the block's data
+// pos: the low 32 bits of the arena byte offset of a 16-byte vector.  Offsets inside one column's data are < 4 GiB, so the drain gets the
+// vector's offset inside the block's data back exactly as pos - (uint32_t)data_off (mod 2^32) without the streaming side reading the column.
+struct ScanCand { uint32_t block, pos; };
 
 // all candidates of one vector: word i matches pattern r => an occurrence may start at pos + 4 i + delta[r]
 template <bool MASKED>
@@ -844,112 +859,124 @@ static __device__ __forceinline__ void scan_vector(const DevProgram& P, const Ba
     }
 }
 
-// One tile of the streaming side.  FULL: the tile lies wholly inside the data, so the four loads of a round go out without bounds predicates at
-// immediate offsets from one pointer; otherwise (a block's last tile) every vector is checked against the end of the data and vectors past it
-// are streamed as zeros.  INPLACE: candidates are verified where they are found instead of being queued (the re-scan of a tile whose
-// candidates did not fit the queue).  Returns true when this lane had a candidate vector that found the queue full.
-// The queueing code is inline on purpose: with a call inside the round loop ptxas parks the loop state (pointer, round counter, block) in local
-// memory around every round (the call ABI pins most of the 48 registers), 6 local loads / stores per round.
-template <bool MASKED, bool FULL, bool INPLACE>
-static __device__ __forceinline__ bool scan_tile(const DevProgram& P, const BatchView& B, const DevColumn& c, const ScanParams& sp, uint32_t b,
-                                                 const uint32_t* __restrict__ row_off8, uint64_t* __restrict__ leaf_bm, ScanCand* s_q, uint32_t* s_cnt, uint32_t tile0) {
-    const uint32_t n = (uint32_t)c.data_len;           // < 4 GiB by construction (upload rejects larger payloads)
-    const uint8_t* __restrict__ data = B.arena + c.data_off;
+// This thread's VL_SCAN_UNROLL vectors of one round of a tile, 16 KiB apart (a warp's requests spread over more L2 slices / HBM channels than
+// adjacent 4 KiB slices would).  A round that lies wholly inside the tile (every round of a full tile) loads at immediate offsets from one
+// pointer without predicates; a round that holds the end of a block's last tile checks each vector and streams the ones past the end as zeros
+// (a zero word can only match a pattern of NUL bytes, rejected by the bounds in scan_vector).  A record with bytes == 0 loads nothing.
+static __device__ __forceinline__ void scan_load_round(uint4 (&v)[VL_SCAN_UNROLL], const BatchView& B, const ScanTile& tl, int round) {
+    const uint32_t base = (uint32_t)round * VL_SCAN_ROUND_BYTES + threadIdx.x * 16;
+    const uint8_t* __restrict__ ptr = B.arena + tl.off + base;
+    if ((uint32_t)(round + 1) * VL_SCAN_ROUND_BYTES + (VL_SCAN_UNROLL - 1) * VL_SCAN_QSTRIDE <= tl.bytes) {   // uniform
+#pragma unroll
+        for (int u = 0; u < VL_SCAN_UNROLL; u++) v[u] = __ldg((const uint4*)(ptr + u * VL_SCAN_QSTRIDE));
+    } else {
+        // payloads keep >= 32 readable bytes past data_len: a vector load that starts inside the tile is always in bounds
+#pragma unroll
+        for (int u = 0; u < VL_SCAN_UNROLL; u++) v[u] = base + u * VL_SCAN_QSTRIDE < tl.bytes ? __ldg((const uint4*)(ptr + u * VL_SCAN_QSTRIDE)) : make_uint4(0, 0, 0, 0);
+    }
+}
+
+// Filter of one round and queueing of its candidate vectors.  `pos` = low 32 bits of the arena offset of the thread's first vector of the
+// round.  Returns true when this lane had a candidate vector that found the queue full.
+// The queueing code is inline on purpose: with a call inside the stream ptxas parks the loop state in local memory around every round.
+template <bool MASKED>
+static __device__ __forceinline__ bool scan_round(const uint4 (&v)[VL_SCAN_UNROLL], const ScanParams& sp, uint32_t b, uint32_t pos, ScanCand* s_q, uint32_t* s_cnt) {
+    static_assert(VL_SCAN_UNROLL == 4, "one ballot per vector index below");
+    // bit u of `hits`: vector u holds a word equal to one of the four patterns (one predicate chain of 16 x setp.eq.or per vector)
+    uint32_t hits = 0;
+#pragma unroll
+    for (int u = 0; u < VL_SCAN_UNROLL; u++) hits |= scan_vector_hit<MASKED>(v[u], sp) << u;
+    if (!__any_sync(0xffffffffu, hits != 0)) return false;
+    // some lane has a candidate: the whole warp reserves queue slots with ONE shared-memory atomic per round (lane 0 adds the number of
+    // candidate vectors of all four vector indices); a lane's slot = the warp's base + the vectors of lower indices + those of lower lanes
     const uint32_t lane = threadIdx.x & 31;
+    const uint32_t b0 = __ballot_sync(0xffffffffu, hits & 1), b1 = __ballot_sync(0xffffffffu, hits & 2), b2 = __ballot_sync(0xffffffffu, hits & 4), b3 = __ballot_sync(0xffffffffu, hits & 8);
+    const uint32_t n0 = __popc(b0), n1 = n0 + __popc(b1), n2 = n1 + __popc(b2), n3 = n2 + __popc(b3);
+    uint32_t at0 = 0;
+    if (lane == 0) at0 = atomicAdd(s_cnt, n3);
+    at0 = __shfl_sync(0xffffffffu, at0, 0);
+    const uint32_t below = (1u << lane) - 1u;
+    const uint32_t bal[4] = {b0, b1, b2, b3}, first[4] = {at0, at0 + n0, at0 + n1, at0 + n2};
     bool overflow = false;
-#pragma unroll 1
-    for (int round = 0; round < VL_SCAN_ROUNDS; round++) {
-        const uint32_t round0 = tile0 + (uint32_t)round * (VL_SCAN_THREADS * 16);
-        if (!FULL && round0 >= n) break;                  // uniform: the whole round lies past the data
-        const uint32_t base = round0 + threadIdx.x * 16;
-        uint4 v[VL_SCAN_UNROLL];
-        if (FULL) {
-            const uint8_t* __restrict__ ptr = data + base;
 #pragma unroll
-            for (int u = 0; u < VL_SCAN_UNROLL; u++) v[u] = __ldg((const uint4*)(ptr + u * VL_SCAN_QSTRIDE));
-        } else {
-#pragma unroll
-            for (int u = 0; u < VL_SCAN_UNROLL; u++) {
-                const uint32_t p = base + u * VL_SCAN_QSTRIDE;
-                // payloads keep >= 32 readable bytes past data_len: a vector load that starts before n is always in bounds
-                v[u] = p < n ? __ldg((const uint4*)(data + p)) : make_uint4(0, 0, 0, 0);
-            }
-        }
-        // bit u of `hits`: vector u holds a word equal to one of the four patterns (one predicate chain of 16 x setp.eq.or per vector)
-        uint32_t hits = 0;
-#pragma unroll
-        for (int u = 0; u < VL_SCAN_UNROLL; u++) hits |= scan_vector_hit<MASKED>(v[u], sp) << u;
-        if (!__any_sync(0xffffffffu, hits != 0)) continue;
-        if (INPLACE) {
-#pragma unroll 1
-            for (int u = 0; u < VL_SCAN_UNROLL; u++) if (hits >> u & 1) scan_vector<MASKED>(P, B, c, sp, b, row_off8, base + u * VL_SCAN_QSTRIDE, leaf_bm);
-            continue;
-        }
-        // some lane has a candidate: the whole warp reserves queue slots with ONE shared-memory atomic per round (lane 0 adds the number of
-        // candidate vectors of all four vector indices); a lane's slot = the warp's base + the vectors of lower indices + those of lower lanes
-        const uint32_t b0 = __ballot_sync(0xffffffffu, hits & 1), b1 = __ballot_sync(0xffffffffu, hits & 2), b2 = __ballot_sync(0xffffffffu, hits & 4), b3 = __ballot_sync(0xffffffffu, hits & 8);
-        const uint32_t n0 = __popc(b0), n1 = n0 + __popc(b1), n2 = n1 + __popc(b2), n3 = n2 + __popc(b3);
-        uint32_t at0 = 0;
-        if (lane == 0) at0 = atomicAdd(s_cnt, n3);
-        at0 = __shfl_sync(0xffffffffu, at0, 0);
-        const uint32_t below = (1u << lane) - 1u;
-        const uint32_t bal[4] = {b0, b1, b2, b3}, first[4] = {at0, at0 + n0, at0 + n1, at0 + n2};
-#pragma unroll
-        for (int u = 0; u < VL_SCAN_UNROLL; u++) {
-            if (!(hits >> u & 1)) continue;
-            const uint32_t at = first[u] + __popc(bal[u] & below);
-            if (at < VL_SCAN_QCAP) s_q[at] = ScanCand{b, base + u * VL_SCAN_QSTRIDE}; else overflow = true;
-        }
+    for (int u = 0; u < VL_SCAN_UNROLL; u++) {
+        if (!(hits >> u & 1)) continue;
+        const uint32_t at = first[u] + __popc(bal[u] & below);
+        if (at < VL_SCAN_QCAP) s_q[at] = ScanCand{b, pos + u * VL_SCAN_QSTRIDE}; else overflow = true;
     }
     return overflow;
 }
+
+// The re-scan of a tile whose candidate vectors did not all fit the queue: every vector of the tile, candidates verified where they are found.
 template <bool MASKED>
-static __device__ __noinline__ bool scan_tail_tile(const DevProgram& P, const BatchView& B, const DevColumn& c, const ScanParams& sp, uint32_t b,
-                                                   const uint32_t* __restrict__ row_off8, uint64_t* __restrict__ leaf_bm, ScanCand* s_q, uint32_t* s_cnt, uint32_t tile0) {
-    return scan_tile<MASKED, false, false>(P, B, c, sp, b, row_off8, leaf_bm, s_q, s_cnt, tile0);
-}
-template <bool MASKED>
-static __device__ __noinline__ void scan_tile_inplace(const DevProgram& P, const BatchView& B, const DevColumn& c, const ScanParams& sp, uint32_t b,
-                                                      const uint32_t* __restrict__ row_off8, uint64_t* __restrict__ leaf_bm, uint32_t tile0) {
-    scan_tile<MASKED, false, true>(P, B, c, sp, b, row_off8, leaf_bm, nullptr, nullptr, tile0);
+static __device__ __noinline__ void scan_tile_inplace(const DevProgram& P, const BatchView& B, int slot, const ScanParams& sp, const ScanTile tl,
+                                                      const uint32_t* __restrict__ row_off8, uint64_t* __restrict__ leaf_bm) {
+    const DevColumn& c = B.cols[(uint64_t)tl.block * B.nfields + slot];
+    const uint32_t tile0 = (uint32_t)(tl.off - c.data_off);
+    for (uint32_t p = threadIdx.x * 16; p < tl.bytes; p += VL_SCAN_ROUND_BYTES) scan_vector<MASKED>(P, B, c, sp, tl.block, row_off8, tile0 + p, leaf_bm);
 }
 template <bool MASKED>
 static __device__ __noinline__ void scan_drain(const DevProgram& P, const BatchView& B, int slot, const ScanParams& sp, const uint32_t* __restrict__ row_off8,
                                                uint64_t* __restrict__ leaf_bm, const ScanCand* s_q, uint32_t count) {
     for (uint32_t i = threadIdx.x; i < count; i += blockDim.x) {
         const ScanCand e = s_q[i];
-        scan_vector<MASKED>(P, B, B.cols[(uint64_t)e.block * B.nfields + slot], sp, e.block, row_off8, e.pos, leaf_bm);
+        const DevColumn& c = B.cols[(uint64_t)e.block * B.nfields + slot];
+        scan_vector<MASKED>(P, B, c, sp, e.block, row_off8, e.pos - (uint32_t)c.data_off, leaf_bm);
     }
 }
 
-// Persistent grid: SMs (132 on an H100) x 5 resident CTAs x 256 threads, each CTA strides over the tile table built by k_plan_leaf.  Per round a thread has
-// four independent LDG.128 in flight, 16 KiB apart (a warp's requests spread over more L2 slices / HBM channels than adjacent 4 KiB slices would).
+static __device__ __forceinline__ ScanTile scan_tile_at(const ScanTile* __restrict__ tiles, uint32_t t, uint32_t ntiles) {   // bytes == 0: no tile
+    if (t >= ntiles) return ScanTile{0, 0, 0};
+    const uint4 r = __ldg((const uint4*)(tiles + t));
+    return ScanTile{(uint64_t)r.y << 32 | r.x, r.z, r.w};
+}
+
+// Persistent grid: SMs (132 on an H100) x VL_SCAN_CTAS resident CTAs x 256 threads, each CTA strides over the tile list built by k_plan_leaf.
+// A CTA's tiles form one software pipeline: the loads of the round VL_SCAN_STAGES - 1 ahead (near the end of a tile: of the next tile) go out
+// before the current round is evaluated, the next tile's record is fetched a whole tile ahead, and the next tile's first rounds are in flight
+// across the end-of-tile barrier and drain.
 template <bool MASKED>
-static __global__ void __launch_bounds__(VL_SCAN_THREADS, 5) k_substr_scan(const __grid_constant__ DevProgram P, const __grid_constant__ BatchView B, int slot, const __grid_constant__ ScanParams sp, const uint32_t* __restrict__ tile_block,
-                                                                           const uint32_t* __restrict__ tile_off, const uint32_t* __restrict__ work_count,
-                                                                           const uint32_t* __restrict__ row_off8, uint64_t* __restrict__ leaf_bm) {
+static __global__ void __launch_bounds__(VL_SCAN_THREADS, VL_SCAN_CTAS) k_substr_scan(const __grid_constant__ DevProgram P, const __grid_constant__ BatchView B, int slot, const __grid_constant__ ScanParams sp,
+                                                                                      const ScanTile* __restrict__ tiles, const uint32_t* __restrict__ work_count,
+                                                                                      const uint32_t* __restrict__ row_off8, uint64_t* __restrict__ leaf_bm) {
     __shared__ ScanCand s_q[VL_SCAN_QCAP];
-    __shared__ uint32_t s_cnt;
+    __shared__ uint32_t s_cnt, s_t, s_ntiles;
+    __shared__ ScanTile s_next;
     if (threadIdx.x == 0) s_cnt = 0;
     __syncthreads();
-    const uint32_t ntiles = work_count[WC_TILES];
+    uint32_t ntiles = work_count[WC_TILES];
+    ScanTile cur = scan_tile_at(tiles, blockIdx.x, ntiles), next = scan_tile_at(tiles, blockIdx.x + gridDim.x, ntiles);
+    uint4 v[VL_SCAN_STAGES][VL_SCAN_UNROLL];
+#pragma unroll
+    for (int s = 0; s < VL_SCAN_STAGES - 1; s++) scan_load_round(v[s], B, cur, s);
     for (uint32_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        const uint32_t b = __ldg(tile_block + t), tile0 = __ldg(tile_off + t);
-        const DevColumn& c = B.cols[(uint64_t)b * B.nfields + slot];
-        bool overflow;
-        if (tile0 + VL_TILE_BYTES <= (uint32_t)c.data_len) overflow = scan_tile<MASKED, true, false>(P, B, c, sp, b, row_off8, leaf_bm, s_q, &s_cnt, tile0);
-        else overflow = scan_tail_tile<MASKED>(P, B, c, sp, b, row_off8, leaf_bm, s_q, &s_cnt, tile0);
+        bool overflow = false;
+#pragma unroll
+        for (int r = 0; r < VL_SCAN_ROUNDS; r++) {
+            const int ahead = r + VL_SCAN_STAGES - 1;
+            if (ahead < VL_SCAN_ROUNDS) scan_load_round(v[ahead % VL_SCAN_STAGES], B, cur, ahead);
+            else scan_load_round(v[ahead % VL_SCAN_STAGES], B, next, ahead - VL_SCAN_ROUNDS);
+            overflow |= scan_round<MASKED>(v[r % VL_SCAN_STAGES], sp, cur.block, (uint32_t)cur.off + (uint32_t)r * VL_SCAN_ROUND_BYTES + threadIdx.x * 16, s_q, &s_cnt);
+        }
         // end of the tile: drain the queue if it is worth a pass of the whole CTA (thread 0 decides; the barrier makes the decision uniform),
         // or if some candidate vector of this tile did not fit
         if (__syncthreads_or((threadIdx.x == 0 && s_cnt >= VL_SCAN_QFLUSH) || overflow)) {
+            // No register of the stream lives across the calls below (the call ABI would park it in local memory): the loop state goes
+            // through shared memory and the rounds already issued for the next tile are issued again afterwards.
+            if (threadIdx.x == 0) { s_t = t; s_ntiles = ntiles; s_next = next; }
             // candidates that did not fit were dropped: the tile is gone over again with verification in place (bits are OR-ed, so the
             // candidates that did make it into the queue and are verified again below change nothing)
-            if (__syncthreads_or(overflow)) scan_tile_inplace<MASKED>(P, B, c, sp, b, row_off8, leaf_bm, tile0);
+            if (__syncthreads_or(overflow)) scan_tile_inplace<MASKED>(P, B, slot, sp, cur, row_off8, leaf_bm);
             scan_drain<MASKED>(P, B, slot, sp, row_off8, leaf_bm, s_q, min(s_cnt, (uint32_t)VL_SCAN_QCAP));
             __syncthreads();
             if (threadIdx.x == 0) s_cnt = 0;
+            t = s_t; ntiles = s_ntiles; next = s_next;
             __syncthreads();
+#pragma unroll
+            for (int s = 0; s < VL_SCAN_STAGES - 1; s++) scan_load_round(v[s], B, next, s);
         }
+        cur = next;
+        next = scan_tile_at(tiles, t + 2 * gridDim.x, ntiles);
     }
     __syncthreads();
     scan_drain<MASKED>(P, B, slot, sp, row_off8, leaf_bm, s_q, min(s_cnt, (uint32_t)VL_SCAN_QCAP));
