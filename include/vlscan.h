@@ -109,9 +109,12 @@ typedef struct vlscan_gen_config {
     uint32_t rows_per_block;
     uint32_t hot_block_permille;
     uint32_t hit_row_permille;
-    uint32_t columns_mask;       /* bit0 _msg, bit1 level, bit2 path, bit3 status; bits 8..11: vocabulary focus for selectivity sweeps
+    uint32_t columns_mask;       /* bit0 _msg, bit1 level, bit2 path, bit3 status; bit4 a timestamps column: row i of the data set at
+                                    VLSCAN_GEN_T0 + i ms (MarshalTypeDeltaConst); bits 8..11: vocabulary focus for selectivity sweeps
                                     (0 = a vocabulary row draws one of the 12 entries uniformly, k = always entry k - 1) */
 } vlscan_gen_config;
+#define VLSCAN_GEN_T0 1700000000000000000ll   /* 2023-11-14T22:13:20Z, nanoseconds */
+#define VLSCAN_GEN_STEP 1000000ll            /* 1 ms between consecutive rows */
 
 /* ---- library / worker context ---------------------------------------------------------------------------------- */
 int vlscan_device_count(void);                               /* number of usable CUDA devices (0 => nothing works)  */
@@ -212,7 +215,8 @@ uint64_t vlscan_batch_device_bytes(const vlscan_batch* batch);
  * identical to what the reference writer path would produce for the same rows; verified against the oracle). */
 int vlscan_batch_generate(vlscan_ctx* ctx, const vlscan_gen_config* cfg, uint64_t block_lo, uint64_t block_hi, vlscan_batch** out);
 
-/* Copy a resident batch back into caller-visible host memory as vlscan_block descriptors (decoded stage).  The
+/* Copy a resident batch back into caller-visible host memory as vlscan_block descriptors (decoded stage, timestamps columns in their plain
+ * marshal types).  The
  * descriptors and payloads live in one library-owned pinned host buffer that stays valid until vlscan_host_blocks_free. */
 typedef struct vlscan_host_blocks vlscan_host_blocks;
 int vlscan_batch_download(vlscan_ctx* ctx, const vlscan_batch* batch, vlscan_host_blocks** out);
@@ -311,6 +315,35 @@ int vlscan_fetch_hits(vlscan_ctx* ctx, uint32_t* out_hit_rows, uint64_t cap, uin
 int vlscan_gather_timestamps(vlscan_ctx* ctx, int64_t* out_timestamps, uint64_t cap, uint64_t* out_hit_offsets);
 int vlscan_gather_values(vlscan_ctx* ctx, const char* field, size_t field_len, uint8_t* out_bytes, uint64_t cap_bytes, uint64_t* out_value_offsets, uint64_t cap_values,
                          uint64_t* out_total_bytes, uint64_t* out_hit_offsets);
+/* ---- the hits histogram: `stats by (_time:step offset off, f1, ...) count() hits` over the selected rows of the last scan ------------------------
+ * The aggregation /select/logsql/hits appends to every query (app/vlselect/logsql/logsql.go:116-219, lib/logstorage/parser.go:407-445), computed
+ * on the device so that only the groups cross PCIe.  Same preconditions as the gather calls: the result of the last vlscan_scan_resident of the
+ * ctx, whose batch must still be alive.  Every block with selected rows must have been staged with its timestamps.
+ *   bucket of a row: truncateTimestamp (lib/logstorage/block_result.go:818-848); step = int64(byStatsField.bucketSize) (<= 0 counts as 1),
+ *     offset = int64(bucketOffset), both in nanoseconds; calendar = VLSCAN_BUCKET_WEEK / _MONTH / _YEAR when bucketSizeStr is "week" / "month" /
+ *     "year" (the week starts on Monday; month and year are UTC calendar units, step is then ignored), VLSCAN_BUCKET_PLAIN otherwise (the
+ *     /hits endpoint always: its step is a duration such as "1w").  int64 arithmetic wraps like Go's.
+ *   group key: the bucket, then the text of every by-field as vlscan_gather_values yields it (typed values formatted, "" for a field a block does
+ *     not have): `200` stored as uint16 in one block and as a string in another is one group.  Keys are compared byte for byte, never by hash.
+ *   by_names: canonical field names ("" = _msg), at most VLSCAN_HITS_MAX_BY; "_time" is rejected.
+ * Output: the groups sorted by bucket, then by the key texts bytewise: out_buckets[g], out_counts[g] (rows), and the texts of group g's by-field
+ * f at out_key_bytes[out_key_offsets[g * nby + f], out_key_offsets[g * nby + f + 1]) (out_key_offsets has cap_groups * nby + 1 entries).
+ * out_info (may be NULL) = {groups, key bytes, selected rows, blocks whose timestamps were decoded}; it is filled also when the call fails because
+ * cap_groups or cap_key_bytes is too small (then nothing else is written).  Blocks whose minimum and maximum timestamps fall into one bucket
+ * are counted without decoding their timestamps. */
+enum { VLSCAN_BUCKET_PLAIN = 0, VLSCAN_BUCKET_WEEK = 1, VLSCAN_BUCKET_MONTH = 2, VLSCAN_BUCKET_YEAR = 3 };
+#define VLSCAN_HITS_MAX_BY 4
+typedef struct vlscan_hits_query {
+    int64_t step, offset;          /* nanoseconds */
+    uint32_t calendar;             /* VLSCAN_BUCKET_*                                                                             */
+    uint32_t nby;                  /* by-fields after _time, <= VLSCAN_HITS_MAX_BY                                                */
+    const char* const* by_names;
+    const size_t* by_name_lens;
+} vlscan_hits_query;
+int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_buckets, uint64_t* out_counts, uint64_t cap_groups, uint8_t* out_key_bytes,
+                      uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t out_info[4]);
+/* The bucket of one timestamp: host build of the routine the hits kernels run per row (truncateTimestamp above).  For tests. */
+int64_t vlscan_truncate_timestamp(int64_t ts, int64_t step, int64_t offset, uint32_t calendar);
 /* Digest of the last scan's bitmaps of the blocks [block_lo, block_hi) of its batch, computed on the device: xor over the blocks of
  * XXH64(the block's bitmap words as little-endian bytes) * (2 * (key_base + block index) + 1).  The oracle reports the same quantity for its own
  * bitmaps, so a bench can check a billion-row scan against the CPU restatement on any block range without moving the bitmaps.  The batch of the

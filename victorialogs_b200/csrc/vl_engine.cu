@@ -1016,6 +1016,16 @@ int vlscan_batch_download(vlscan_ctx* ctx, const vlscan_batch* batch, vlscan_hos
         }
         first[batch->nblocks] = hb->cols.size();
         for (uint64_t b = 0; b < batch->nblocks; b++) { hb->blocks[b].rows = batch->h_rows[b]; hb->blocks[b].ncols = (uint32_t)(first[b + 1] - first[b]); hb->blocks[b].cols = hb->cols.data() + first[b]; }
+        if (batch->has_ts && batch->nblocks) {   // the timestamps columns, in their plain marshal types (ZSTD ones were inflated at upload)
+            std::vector<DevTimestamps> ts(batch->nblocks);
+            VL_CUDA(cudaMemcpy(ts.data(), batch->ts.p, ts.size() * sizeof(DevTimestamps), cudaMemcpyDeviceToHost));
+            for (uint64_t b = 0; b < batch->nblocks; b++) {
+                if (!ts[b].mt) continue;
+                vlscan_block& blk = hb->blocks[b];
+                blk.ts_marshal_type = ts[b].mt; blk.timestamps = base + ts[b].off; blk.timestamps_len = ts[b].len;
+                blk.min_timestamp = ts[b].first; blk.max_timestamp = ts[b].max;
+            }
+        }
     });
     if (rc) { if (hb->pinned) cudaFreeHost(hb->pinned); delete hb; return rc; }
     *out = hb;
@@ -1319,6 +1329,44 @@ int vlscan_gather_timestamps(vlscan_ctx* ctx, int64_t* out_timestamps, uint64_t 
     });
 }
 
+// batch field slot of a canonical field name, -1 when no block of the batch has it
+static int field_slot(const vlscan_batch* b, const std::string& name) {
+    for (uint32_t s = 0; s < b->nfields; s++) if (b->field_names[s] == name) return (int)s;
+    return -1;
+}
+// row offsets of the strings blocks with hits in column `slot` (kept from the scan where it already computed them)
+static const uint32_t* hit_row_offsets(vlscan_ctx* ctx, int slot) {
+    if (slot < 0) return nullptr;
+    BatchView B = ctx->last_batch->view();
+    uint32_t* wc = ctx->work_count.as<uint32_t>();
+    VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
+    k_hit_blocks_list<<<cdiv(B.nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), slot, 0, ctx->lens_blocks.as<uint32_t>(), wc); launch_check(ctx);
+    uint8_t* ready = ctx->ready[slot].as<uint8_t>();
+    if (!ctx->ready_cleared[slot]) { VL_CUDA(cudaMemsetAsync(ready, 0, B.nblocks, ctx->stream)); ctx->ready_cleared[slot] = 1; }
+    k_lens_offsets<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(B, slot, ctx->lens_blocks.as<uint32_t>(), wc, ctx->row_off8[slot].as<uint32_t>(), ready, ctx->gstat.as<unsigned long long>()); launch_check(ctx);
+    return ctx->row_off8[slot].as<uint32_t>();
+}
+// texts of column `slot` in the n rows (rows[i], blocks[i]): their lengths and exclusive offsets go to ctx->glens / ctx->goffs (goffs[n] = the
+// total, also returned; synchronises), then text_bytes writes the bytes to ctx->gout
+static uint64_t text_offsets(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint32_t* rows, const uint32_t* blocks, uint64_t n) {
+    BatchView B = ctx->last_batch->view();
+    const uint64_t ntiles = cdiv(n, VL_SCAN_TILE);
+    ctx->glens.ensure(n * 4); ctx->goffs.ensure((n + 1) * 8); ctx->gtiles.ensure((ntiles + 1) * 8);
+    k_gather_values<<<cdiv(n, 128), 128, 0, ctx->stream>>>(B, slot, rows, blocks, n, ro, 0, ctx->glens.as<uint32_t>(), nullptr, nullptr, ctx->gstat.as<unsigned long long>()); launch_check(ctx);
+    k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(ctx->glens.as<uint32_t>(), n, ctx->gtiles.as<unsigned long long>(), nullptr, 0); launch_check(ctx);
+    k_scan_tile_sums<<<1, 1024, 0, ctx->stream>>>(ctx->gtiles.as<unsigned long long>(), ntiles, ctx->goffs.as<unsigned long long>() + n); launch_check(ctx);
+    k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(ctx->glens.as<uint32_t>(), n, ctx->gtiles.as<unsigned long long>(), ctx->goffs.as<unsigned long long>(), 1); launch_check(ctx);
+    uint64_t total = 0;
+    VL_CUDA(cudaMemcpyAsync(&total, ctx->goffs.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    check_gather_errors(ctx);
+    return total;
+}
+static void text_bytes(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint32_t* rows, const uint32_t* blocks, uint64_t n, uint64_t total) {
+    ctx->gout.ensure(std::max<uint64_t>(total, 16));
+    k_gather_values<<<cdiv(n, 128), 128, 0, ctx->stream>>>(ctx->last_batch->view(), slot, rows, blocks, n, ro, 1, nullptr, ctx->goffs.as<uint64_t>(), ctx->gout.as<uint8_t>(), ctx->gstat.as<unsigned long long>());
+    launch_check(ctx);
+}
+
 int vlscan_gather_values(vlscan_ctx* ctx, const char* field, size_t field_len, uint8_t* out_bytes, uint64_t cap_bytes, uint64_t* out_value_offsets, uint64_t cap_values,
                          uint64_t* out_total_bytes, uint64_t* out_hit_offsets) {
     if (out_total_bytes) *out_total_bytes = 0;
@@ -1327,39 +1375,128 @@ int vlscan_gather_values(vlscan_ctx* ctx, const char* field, size_t field_len, u
         if (n > cap_values) throw BadInput("value offsets buffer too small");
         if (out_value_offsets) out_value_offsets[0] = 0;
         if (!n) return;
-        const vlscan_batch* b = ctx->last_batch;
-        BatchView B = b->view();
         std::string name(field, field_len); if (name.empty()) name = "_msg";   // getCanonicalColumnName
-        int slot = -1;
-        for (uint32_t s2 = 0; s2 < b->nfields; s2++) if (b->field_names[s2] == name) slot = (int)s2;
-        uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* lens_blocks = ctx->lens_blocks.as<uint32_t>();
-        unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
-        const uint32_t* ro = nullptr;
-        if (slot >= 0) {   // row offsets of the strings blocks with hits (kept from the scan where it already computed them)
-            VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
-            k_hit_blocks_list<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), slot, 0, lens_blocks, wc); launch_check(ctx);
-            uint8_t* ready = ctx->ready[slot].as<uint8_t>();
-            if (!ctx->ready_cleared[slot]) { VL_CUDA(cudaMemsetAsync(ready, 0, B.nblocks, ctx->stream)); ctx->ready_cleared[slot] = 1; }
-            k_lens_offsets<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(B, slot, lens_blocks, wc, ctx->row_off8[slot].as<uint32_t>(), ready, gstat); launch_check(ctx);
-            ro = ctx->row_off8[slot].as<uint32_t>();
-        }
-        const uint64_t ntiles = cdiv(n, VL_SCAN_TILE);
-        ctx->glens.ensure(n * 4); ctx->goffs.ensure((n + 1) * 8); ctx->gtiles.ensure((ntiles + 1) * 8);
-        k_gather_values<<<cdiv(n, 128), 128, 0, ctx->stream>>>(B, slot, ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), n, ro, 0, ctx->glens.as<uint32_t>(), nullptr, nullptr, gstat); launch_check(ctx);
-        k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(ctx->glens.as<uint32_t>(), n, ctx->gtiles.as<unsigned long long>(), nullptr, 0); launch_check(ctx);
-        k_scan_tile_sums<<<1, 1024, 0, ctx->stream>>>(ctx->gtiles.as<unsigned long long>(), ntiles, ctx->goffs.as<unsigned long long>() + n); launch_check(ctx);
-        k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(ctx->glens.as<uint32_t>(), n, ctx->gtiles.as<unsigned long long>(), ctx->goffs.as<unsigned long long>(), 1); launch_check(ctx);
-        uint64_t total = 0;
-        VL_CUDA(cudaMemcpyAsync(&total, ctx->goffs.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
-        check_gather_errors(ctx);
+        const int slot = field_slot(ctx->last_batch, name);
+        const uint32_t* ro = hit_row_offsets(ctx, slot);
+        const uint32_t* rows = ctx->hits.as<uint32_t>(); const uint32_t* blocks = ctx->hit_block.as<uint32_t>();
+        const uint64_t total = text_offsets(ctx, slot, ro, rows, blocks, n);
         if (out_total_bytes) *out_total_bytes = total;
         if (total > cap_bytes) throw BadInput("values buffer too small (the needed size is reported)");
-        ctx->gout.ensure(std::max<uint64_t>(total, 16));
-        k_gather_values<<<cdiv(n, 128), 128, 0, ctx->stream>>>(B, slot, ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), n, ro, 1, nullptr, ctx->goffs.as<uint64_t>(), ctx->gout.as<uint8_t>(), gstat); launch_check(ctx);
+        text_bytes(ctx, slot, ro, rows, blocks, n, total);
         if (out_value_offsets) VL_CUDA(cudaMemcpyAsync(out_value_offsets, ctx->goffs.p, (n + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
         if (total) VL_CUDA(cudaMemcpyAsync(out_bytes, ctx->gout.p, total, cudaMemcpyDeviceToHost, ctx->stream));
         VL_CUDA(cudaStreamSynchronize(ctx->stream));
     });
+}
+
+static_assert(VLSCAN_HITS_MAX_BY == VL_HITS_MAX_BY, "the ABI's and the kernels' by-field limits differ");
+int64_t vlscan_truncate_timestamp(int64_t ts, int64_t step, int64_t offset, uint32_t calendar) { return vl::truncate_timestamp(ts, step, offset, calendar); }
+
+int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_buckets, uint64_t* out_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes,
+                      uint64_t* out_key_offsets, uint64_t out_info[4]) {
+    uint64_t info[4] = {0, 0, 0, 0};   // groups, key bytes, selected rows, blocks whose timestamps were decoded
+    const int rc = guarded(ctx, [&] {
+        if (!q) throw BadInput("no hits query");
+        if (q->calendar > VLSCAN_BUCKET_YEAR) throw BadInput("unknown calendar bucket kind");
+        if (q->nby > VLSCAN_HITS_MAX_BY) throw BadInput("too many by-fields for the hits aggregation (at most VLSCAN_HITS_MAX_BY = 4)");
+        std::vector<std::string> names;
+        for (uint32_t f = 0; f < q->nby; f++) {
+            std::string n(q->by_names[f], q->by_name_lens[f]);
+            if (n.empty()) n = "_msg";   // getCanonicalColumnName
+            if (n == "_time") throw BadInput("`_time` cannot be a by-field of the hits aggregation: it is the bucket");
+            names.push_back(n);
+        }
+        if (!ctx) throw BadInput("vlscan_hits_stats needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
+        const uint64_t n = build_hit_list(ctx, nullptr);
+        if (n >= 0xFFFFFFFFull) throw BadInput("more than 2^32 - 2 selected rows in one batch");
+        info[2] = n;
+        if (out_key_offsets) out_key_offsets[0] = 0;
+        if (!n) return;
+        const vlscan_batch* b = ctx->last_batch;
+        BatchView B = b->view();
+        HitsQuery hq;
+        memset(&hq, 0, sizeof hq);
+        hq.step = q->step; hq.offset = q->offset; hq.calendar = q->calendar; hq.nby = q->nby;
+        for (uint32_t f = 0; f < q->nby; f++) { hq.slot[f] = field_slot(b, names[f]); hq.row_off8[f] = hit_row_offsets(ctx, hq.slot[f]); }
+        // buckets of the blocks; timestamps decoded only where a block spans several buckets
+        unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
+        uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* row_blocks = ctx->row_blocks.as<uint32_t>();
+        ctx->hblk.ensure(b->nblocks * 9 + 16);
+        long long* blk_bucket = ctx->hblk.as<long long>(); uint8_t* blk_multi = ctx->hblk.as<uint8_t>() + b->nblocks * 8;
+        VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
+        k_hits_classify<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), hq, blk_bucket, blk_multi, row_blocks, wc, gstat); launch_check(ctx);
+        ctx->ts_vals.ensure(b->nwords * 64 * 8);
+        k_ts_decode_list<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(B, row_blocks, wc, ctx->ts_vals.as<unsigned long long>(), gstat); launch_check(ctx);
+        uint32_t decoded = 0;
+        VL_CUDA(cudaMemcpyAsync(&decoded, wc + WC_ROW, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        HitsView V{ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), blk_bucket, blk_multi, ctx->ts_vals.as<unsigned long long>()};
+        // the group table: starts small, grows by 8x while a pass overflows; at 2 x the hit count it cannot overflow
+        uint64_t max_cap = 1024; while (max_cap < 2 * n) max_cap <<= 1;
+        uint64_t cap = std::min<uint64_t>(max_cap, 1 << 14);
+        HitsTable T;
+        unsigned long long state[3];
+        for (;;) {
+            ctx->htab.ensure(cap * 16 + 32);
+            T.tags = ctx->htab.as<unsigned long long>(); T.cnt = T.tags + cap; T.state = T.cnt + cap;
+            T.mask = cap - 1; T.limit = cap == max_cap ? cap : cap / 2;
+            VL_CUDA(cudaMemsetAsync(T.tags, 0, cap * 16 + 32, ctx->stream));
+            k_hits_group<<<(unsigned)std::min<uint64_t>(b->nblocks, (uint64_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(B, hq, V, T, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat);
+            launch_check(ctx);
+            VL_CUDA(cudaMemcpyAsync(state, T.state, sizeof state, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaStreamSynchronize(ctx->stream));
+            if (!state[1]) break;
+            if (cap == max_cap) throw BadInput("hits aggregation: group table overflow");
+            cap = std::min(cap * 8, max_cap);
+        }
+        check_gather_errors(ctx);
+        const uint64_t G = state[0];
+        info[0] = G; info[3] = decoded;
+        // the groups, then the texts of their representatives only
+        ctx->hgrp.ensure(G * 24 + 64);
+        long long* buckets = ctx->hgrp.as<long long>(); unsigned long long* counts = (unsigned long long*)(buckets + G);
+        uint32_t* rep_rows = (uint32_t*)(counts + G); uint32_t* rep_blocks = rep_rows + G;
+        k_hits_emit<<<cdiv(cap, 256), 256, 0, ctx->stream>>>(B, hq, V, T, rep_rows, rep_blocks, buckets, counts); launch_check(ctx);
+        std::vector<int64_t> hb(G); std::vector<uint64_t> hc(G);
+        VL_CUDA(cudaMemcpyAsync(hb.data(), buckets, G * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaMemcpyAsync(hc.data(), counts, G * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        std::vector<std::vector<uint64_t>> toffs(q->nby); std::vector<std::vector<uint8_t>> tbytes(q->nby);
+        uint64_t key_bytes = 0;
+        for (uint32_t f = 0; f < q->nby; f++) {
+            const uint64_t total = text_offsets(ctx, hq.slot[f], hq.row_off8[f], rep_rows, rep_blocks, G);
+            key_bytes += total;
+            toffs[f].resize(G + 1); tbytes[f].resize(total);
+            text_bytes(ctx, hq.slot[f], hq.row_off8[f], rep_rows, rep_blocks, G, total);
+            VL_CUDA(cudaMemcpyAsync(toffs[f].data(), ctx->goffs.p, (G + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+            if (total) VL_CUDA(cudaMemcpyAsync(tbytes[f].data(), ctx->gout.p, total, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaStreamSynchronize(ctx->stream));
+        }
+        VL_CUDA(cudaStreamSynchronize(ctx->stream));
+        info[1] = key_bytes;
+        if (G > cap_groups) throw BadInput("hits groups buffer too small (the needed size is reported)");
+        if (key_bytes > cap_key_bytes) throw BadInput("hits key bytes buffer too small (the needed size is reported)");
+        if (!out_buckets || !out_counts || (q->nby && (!out_key_offsets || (key_bytes && !out_key_bytes)))) throw BadInput("hits output buffer missing");
+        // sorted by bucket, then by the key texts bytewise
+        std::vector<uint64_t> order(G);
+        for (uint64_t g = 0; g < G; g++) order[g] = g;
+        auto text = [&](uint32_t f, uint64_t g) { return std::string_view((const char*)tbytes[f].data() + toffs[f][g], toffs[f][g + 1] - toffs[f][g]); };
+        std::sort(order.begin(), order.end(), [&](uint64_t x, uint64_t y) {
+            if (hb[x] != hb[y]) return hb[x] < hb[y];
+            for (uint32_t f = 0; f < q->nby; f++) { const int c = text(f, x).compare(text(f, y)); if (c) return c < 0; }
+            return false;
+        });
+        uint64_t o = 0;
+        for (uint64_t i = 0; i < G; i++) {
+            const uint64_t g = order[i];
+            out_buckets[i] = hb[g]; out_counts[i] = hc[g];
+            for (uint32_t f = 0; f < q->nby; f++) {
+                const std::string_view t = text(f, g);
+                memcpy(out_key_bytes + o, t.data(), t.size()); o += t.size();
+                out_key_offsets[i * q->nby + f + 1] = o;
+            }
+        }
+    });
+    if (out_info) memcpy(out_info, info, sizeof info);
+    return rc;
 }
 
 int vlscan_result_digest(vlscan_ctx* ctx, uint64_t block_lo, uint64_t block_hi, uint64_t key_base, uint64_t* out_digest) {

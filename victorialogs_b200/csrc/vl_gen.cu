@@ -8,6 +8,8 @@
 //   * `level`: dict column, ids in first-seen order (values_encoder.go:1224-1241), no bloom (block.go:159-168),
 //   * `status`: uint16 column, big-endian values + min/max (values_encoder.go:1168-1222),
 //   * bloom filters: 16 bits per unique token hash, 6 probes, big-endian u64 words (bloomfilter.go:83-121).
+//   * timestamps (columns_mask bit 4): row i of the data set at VLSCAN_GEN_T0 + i * VLSCAN_GEN_STEP, a constant delta, so every block is
+//     MarshalTypeDeltaConst: the varint of the delta and nothing else (vm/lib/encoding/encoding.go:119-130).
 // tests/test_gpu_gen.py checks the output byte-for-byte against the CPU oracle's restatement of that writer path.
 //
 // Supported envelope (anything else is refused with an error instead of silently diverging from the writer):
@@ -263,6 +265,10 @@ extern "C" int vlscan_batch_generate(vlscan_ctx* ctx, const vlscan_gen_config* c
         std::vector<DevColumn> cols((size_t)nb * bt->nfields); memset(cols.data(), 0, cols.size() * sizeof(DevColumn));
         std::vector<GenPlan> plans(nb); memset(plans.data(), 0, plans.size() * sizeof(GenPlan));
         uint64_t cursor = 16;
+        std::vector<DevTimestamps> tsv((c.columns_mask & 16) ? nb : 0);
+        if (!tsv.empty()) memset(tsv.data(), 0, tsv.size() * sizeof(DevTimestamps));
+        std::vector<uint8_t> ts_varint;
+        for (uint64_t u = (uint64_t)VLSCAN_GEN_STEP << 1; ; u >>= 7) { if (u < 0x80) { ts_varint.push_back((uint8_t)u); break; } ts_varint.push_back((uint8_t)(u | 0x80)); }
         for (uint32_t j = 0; j < nb; j++) {
             const GenInfo& gi = info[j]; GenPlan& pl = plans[j]; uint32_t R = rows[j];
             if (gi.overflow) throw BadInput("generator: token set overflow");
@@ -299,6 +305,12 @@ extern "C" int vlscan_batch_generate(vlscan_ctx* ctx, const vlscan_gen_config* c
                 if (gi.path_distinct <= 8) throw BadInput("generator: `path` would become a dict / const column in this block");
                 strings_col(slot_of[2], gi.path_bytes, gi.path_minlen, gi.path_maxlen, gi.path_tokens, &pl.path_lens, &pl.path_data, &pl.path_bloom, &pl.path_bloom_words, &pl.path_lens_const);
             }
+            if (c.columns_mask & 16) {   // encoding.MarshalVarInt64(delta): zig-zag, then unsigned varint
+                DevTimestamps& t = tsv[j];
+                const uint64_t first = (uint64_t)VLSCAN_GEN_T0 + ((block_lo + j) * c.rows_per_block) * (uint64_t)VLSCAN_GEN_STEP;
+                t.first = (int64_t)first; t.max = (int64_t)(first + (uint64_t)(R - 1) * VLSCAN_GEN_STEP);
+                t.mt = MT_DELTA_CONST; t.len = (uint32_t)ts_varint.size(); t.off = arena_reserve(cursor, ts_varint.size());
+            }
             if (slot_of[3] >= 0) {
                 int present = __builtin_popcount(gi.status_mask);
                 if (present <= 8) throw BadInput("generator: `status` would become a dict / const column in this block");
@@ -328,6 +340,7 @@ extern "C" int vlscan_batch_generate(vlscan_ctx* ctx, const vlscan_gen_config* c
             for (uint32_t j = 0; j < nb; j++) {
                 if (slot_of[1] >= 0) pokes.emplace_back(cols[(size_t)j * bt->nfields + slot_of[1]].lens_off, (uint8_t)1);
                 if (slot_of[3] >= 0) pokes.emplace_back(cols[(size_t)j * bt->nfields + slot_of[3]].lens_off, (uint8_t)2);
+                if (!tsv.empty()) for (size_t k = 0; k < ts_varint.size(); k++) pokes.emplace_back(tsv[j].off + k, ts_varint[k]);
             }
             if (!pokes.empty()) {
                 // batch the single-byte writes: build a sparse host image chunk by chunk would be wasteful; use a small kernel-free approach
@@ -341,6 +354,12 @@ extern "C" int vlscan_batch_generate(vlscan_ctx* ctx, const vlscan_gen_config* c
                 VL_CUDA(cudaStreamSynchronize(ctx->stream));
                 d_offs.release(); d_vals.release();
             }
+        }
+        if (!tsv.empty()) {
+            bt->ts.ensure(tsv.size() * sizeof(DevTimestamps));
+            VL_CUDA(cudaMemcpyAsync(bt->ts.p, tsv.data(), tsv.size() * sizeof(DevTimestamps), cudaMemcpyHostToDevice, ctx->stream));
+            VL_CUDA(cudaStreamSynchronize(ctx->stream));
+            bt->has_ts = true;
         }
         bt->note_columns(cols);
         finish_batch_layout(ctx, bt, rows);

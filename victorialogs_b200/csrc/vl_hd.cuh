@@ -420,4 +420,47 @@ VL_HDN int fmt_f64(uint8_t* buf, uint64_t bits) {
     return n;
 }
 
+// ---- `_time` buckets of `stats by (_time:step offset off)`: truncateTimestamp (lib/logstorage/block_result.go:818-848) -------------------
+// Go's int64 arithmetic wraps, so every sum and product here is done on uint64.  Month / year buckets go through the UTC civil date
+// (truncateTimestampToMonth / ToYear :2641-2649, time.Date(...).UnixNano(), which wraps the same way near 1677 and 2262).
+enum { BUCKET_PLAIN = 0, BUCKET_WEEK = 1, BUCKET_MONTH = 2, BUCKET_YEAR = 3 };
+static const int64_t kNsPerDay = 86400ll * 1000000000ll;
+VL_HD int64_t days_from_civil(int64_t y, uint32_t m, uint32_t d) {   // proleptic Gregorian, days since 1970-01-01
+    y -= m <= 2;
+    const int64_t era = (y >= 0 ? y : y - 399) / 400;
+    const int64_t yoe = y - era * 400;
+    const int64_t doy = (153 * (m > 2 ? m - 3 : m + 9) + 2) / 5 + d - 1;
+    const int64_t doe = yoe * 365 + yoe / 4 - yoe / 100 + doy;
+    return era * 146097 + doe - 719468;
+}
+VL_HD void civil_from_days(int64_t z, int64_t* y, uint32_t* m) {
+    z += 719468;
+    const int64_t era = (z >= 0 ? z : z - 146096) / 146097;
+    const int64_t doe = z - era * 146097;
+    const int64_t yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;
+    const int64_t doy = doe - (365 * yoe + yoe / 4 - yoe / 100);
+    const int64_t mp = (5 * doy + 2) / 153;
+    *m = (uint32_t)(mp < 10 ? mp + 3 : mp - 9);
+    *y = yoe + era * 400 + (*m <= 2);
+}
+// step <= 0 counts as 1 (getBucketedTimestampValues :763-766); `calendar` is BUCKET_*
+VL_HD int64_t truncate_timestamp(int64_t ts, int64_t step, int64_t offset, uint32_t calendar) {
+    if (step <= 0) step = 1;
+    uint64_t off = (uint64_t)offset;
+    if (calendar == BUCKET_WEEK) off += 4ull * (uint64_t)kNsPerDay;   // weeks start on Monday
+    const uint64_t t = (uint64_t)ts - off;
+    const int64_t st = (int64_t)t;
+    if (calendar == BUCKET_MONTH || calendar == BUCKET_YEAR) {
+        int64_t days = st / kNsPerDay;
+        if (st % kNsPerDay < 0) days--;
+        int64_t y; uint32_t m;
+        civil_from_days(days, &y, &m);
+        const int64_t first = days_from_civil(y, calendar == BUCKET_YEAR ? 1 : m, 1);
+        return (int64_t)((uint64_t)first * (uint64_t)kNsPerDay + off);
+    }
+    int64_t r = st % step;
+    if (r < 0) r += step;
+    return (int64_t)(t - (uint64_t)r + off);
+}
+
 }  // namespace vl

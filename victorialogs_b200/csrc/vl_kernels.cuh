@@ -1344,14 +1344,12 @@ static __global__ void k_gather_ts(BatchView B, const uint32_t* __restrict__ hit
     const uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (h < nhits) out[h] = (long long)ts_vals[B.blk_word_off[hit_block[h]] * 64 + hits[h]];
 }
-// The value of column `slot` in one row as a string.  pass 0: lens[h] = its length; pass 1: the bytes go to out + offs[h].
-static __global__ void k_gather_values(BatchView B, int slot, const uint32_t* __restrict__ hits, const uint32_t* __restrict__ hit_block, uint64_t nhits, const uint32_t* __restrict__ row_off8,
-                                       int pass, uint32_t* __restrict__ lens_out, const uint64_t* __restrict__ offs, uint8_t* __restrict__ out, unsigned long long* __restrict__ stats) {
-    const uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (h >= nhits) return;
-    const uint32_t b = hit_block[h], r = hits[h];
+// The value of column `slot` (-1: a field the batch lacks) in row r of block b as blockResultColumn.getValues yields it: row bytes of a strings
+// column, the dictionary entry, the text form of a typed value (formatted into buf, VL_FMT_F64_MAX bytes), the const value, "" for a field the
+// block does not have.  row_off8: k_lens_offsets of the slot (strings columns with per-row lens items).  Returns the length, *out the bytes.
+static __device__ uint32_t value_text(const BatchView& B, int slot, uint32_t b, uint32_t r, const uint32_t* __restrict__ row_off8, uint8_t* buf, const uint8_t** out,
+                                      unsigned long long* __restrict__ stats) {
     const uint8_t* src = nullptr; uint32_t len = 0;
-    uint8_t buf[VL_FMT_F64_MAX];
     if (slot >= 0) {
         const DevColumn& c = B.cols[(uint64_t)b * B.nfields + slot];
         if (c.kind == COL_CONST) { src = B.hdr + c.meta_off; len = c.meta_len; }
@@ -1379,6 +1377,17 @@ static __global__ void k_gather_values(BatchView B, int slot, const uint32_t* __
             }
         }
     }
+    *out = src;
+    return len;
+}
+// The value of column `slot` in one row as a string.  pass 0: lens[h] = its length; pass 1: the bytes go to out + offs[h].
+static __global__ void k_gather_values(BatchView B, int slot, const uint32_t* __restrict__ hits, const uint32_t* __restrict__ hit_block, uint64_t nhits, const uint32_t* __restrict__ row_off8,
+                                       int pass, uint32_t* __restrict__ lens_out, const uint64_t* __restrict__ offs, uint8_t* __restrict__ out, unsigned long long* __restrict__ stats) {
+    const uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= nhits) return;
+    uint8_t buf[VL_FMT_F64_MAX];
+    const uint8_t* src;
+    const uint32_t len = value_text(B, slot, hit_block[h], hits[h], row_off8, buf, &src, stats);
     if (pass == 0) { lens_out[h] = len; return; }
     uint8_t* d = out + offs[h];
     for (uint32_t k = 0; k < len; k++) d[k] = src[k];
@@ -1566,6 +1575,169 @@ static __global__ void k_bitmap_digest(BatchView B, const uint64_t* __restrict__
 #pragma unroll
     for (int s = 16; s; s >>= 1) d ^= __shfl_xor_sync(0xffffffffu, d, s);
     if (lane_id() == 0 && d) atomicXor(out, d);
+}
+
+// ---- `stats by (_time:step offset off, f1, ...) count()` over the selected rows: the aggregation of /select/logsql/hits --------------------------
+// (app/vlselect/logsql/logsql.go:116-219 builds it, lib/logstorage/block_result.go:760-848 buckets `_time`).  A group is (bucket, the text of every
+// by-field as value_text yields it).  Groups live in an open-addressing table whose slot holds only a 64-bit tag: the high half of the key's hash
+// and 1 + the index of a representative hit.  A key is found by comparing the bucket and the texts with the representative's, byte for byte,
+// so two keys share a slot only when they are equal: a hash collision costs a probe, never a wrong count.  A hit insert that would claim a slot
+// beyond the table's load limit raises the overflow flag; the host then grows the table and runs the pass again.
+#define VL_HITS_MAX_BY 4
+#define VL_HITS_CODES 4096   // (block, dict entry) pre-aggregation: at most 8 dict entries per by-field, so 8^VL_HITS_MAX_BY codes
+struct HitsQuery {
+    int64_t step, offset;
+    uint32_t calendar, nby;
+    int slot[VL_HITS_MAX_BY];                   // batch field slot of every by-field; -1: no block of the batch has it
+    const uint32_t* row_off8[VL_HITS_MAX_BY];   // k_lens_offsets of that slot
+};
+struct HitsView {
+    const uint32_t* hits; const uint32_t* hit_block;                 // build_hit_list
+    const long long* blk_bucket; const uint8_t* blk_multi;           // k_hits_classify
+    const unsigned long long* ts_vals;                               // k_ts_decode_list of the multi-bucket blocks
+};
+struct HitsTable {
+    unsigned long long* tags;    // [mask + 1]: 0 = empty, else (key hash >> 32) << 32 | (representative hit + 1)
+    unsigned long long* cnt;     // [mask + 1]
+    unsigned long long* state;   // [0] slots claimed, [1] overflow, [2] groups emitted
+    uint64_t mask, limit;
+};
+
+// Blocks with hits: the buckets of their minimum and maximum timestamps.  Where they are equal every row of the block is in that bucket (the
+// fast path of getBucketedTimestampValues :769-783) and the timestamps are never decoded; the others go into the decode list.
+static __global__ void k_hits_classify(BatchView B, const uint32_t* __restrict__ counts, HitsQuery q, long long* __restrict__ blk_bucket, uint8_t* __restrict__ blk_multi,
+                                       uint32_t* __restrict__ row_blocks, uint32_t* __restrict__ work_count, unsigned long long* __restrict__ stats) {
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B.nblocks || counts[b] == 0) return;
+    if (!B.ts || B.ts[b].mt == 0) { blk_bucket[b] = 0; blk_multi[b] = 0; atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_NO_TIMESTAMPS); return; }
+    const int64_t lo = truncate_timestamp(B.ts[b].first, q.step, q.offset, q.calendar), hi = truncate_timestamp(B.ts[b].max, q.step, q.offset, q.calendar);
+    blk_bucket[b] = lo; blk_multi[b] = lo != hi;
+    if (lo != hi) row_blocks[atomicAdd(&work_count[WC_ROW], 1u)] = b;
+}
+static __device__ __forceinline__ int64_t hit_bucket(const BatchView& B, const HitsQuery& q, const HitsView& V, uint32_t b, uint32_t r) {
+    return V.blk_multi[b] ? truncate_timestamp((int64_t)V.ts_vals[B.blk_word_off[b] * 64 + r], q.step, q.offset, q.calendar) : (int64_t)V.blk_bucket[b];
+}
+static __device__ __forceinline__ uint64_t mix64(uint64_t z) { z ^= z >> 30; z *= 0xBF58476D1CE4E5B9ULL; z ^= z >> 27; z *= 0x94D049BB133111EBULL; return z ^ (z >> 31); }
+static __device__ uint64_t hits_key_hash(const BatchView& B, const HitsQuery& q, int64_t bucket, uint32_t b, uint32_t r, unsigned long long* stats) {
+    uint64_t h = mix64((uint64_t)bucket);
+    uint8_t buf[VL_FMT_F64_MAX];
+    for (uint32_t f = 0; f < q.nby; f++) {
+        const uint8_t* src;
+        const uint32_t len = value_text(B, q.slot[f], b, r, q.row_off8[f], buf, &src, stats);
+        h = (h ^ len) * 0x100000001B3ull;
+        for (uint32_t k = 0; k < len; k++) h = (h ^ src[k]) * 0x100000001B3ull;
+        h = mix64(h);
+    }
+    return h;
+}
+static __device__ bool hits_same_texts(const BatchView& B, const HitsQuery& q, uint32_t b1, uint32_t r1, uint32_t b2, uint32_t r2, unsigned long long* stats) {
+    uint8_t buf1[VL_FMT_F64_MAX], buf2[VL_FMT_F64_MAX];
+    for (uint32_t f = 0; f < q.nby; f++) {
+        const uint8_t *s1, *s2;
+        const uint32_t l1 = value_text(B, q.slot[f], b1, r1, q.row_off8[f], buf1, &s1, stats), l2 = value_text(B, q.slot[f], b2, r2, q.row_off8[f], buf2, &s2, stats);
+        if (l1 != l2) return false;
+        for (uint32_t k = 0; k < l1; k++) if (s1[k] != s2[k]) return false;
+    }
+    return true;
+}
+// add `c` rows with the key of hit `hit` = row r of block b, whose bucket is `bucket`
+static __device__ void hits_insert(const BatchView& B, const HitsQuery& q, const HitsView& V, const HitsTable& T, int64_t bucket, uint64_t hit, uint32_t b, uint32_t r, uint64_t c,
+                                   unsigned long long* stats) {
+    if (*(volatile unsigned long long*)&T.state[1]) return;
+    const uint64_t hash = hits_key_hash(B, q, bucket, b, r, stats);
+    const unsigned long long tag = (hash & 0xFFFFFFFF00000000ull) | (hit + 1);
+    uint64_t slot = hash & T.mask;
+    for (uint64_t probe = 0; probe <= T.mask; probe++, slot = (slot + 1) & T.mask) {
+        unsigned long long cur = *(volatile unsigned long long*)&T.tags[slot];
+        if (cur == 0) {
+            cur = atomicCAS(&T.tags[slot], 0ull, tag);
+            if (cur == 0) {
+                if (atomicAdd(&T.state[0], 1ull) >= T.limit) atomicExch(&T.state[1], 1ull);
+                atomicAdd(&T.cnt[slot], (unsigned long long)c);
+                return;
+            }
+        }
+        if ((cur >> 32) != (hash >> 32)) continue;
+        const uint64_t rep = (cur & 0xFFFFFFFFull) - 1;
+        const uint32_t rb = V.hit_block[rep], rr = V.hits[rep];
+        if (hit_bucket(B, q, V, rb, rr) == bucket && hits_same_texts(B, q, b, r, rb, rr, stats)) { atomicAdd(&T.cnt[slot], (unsigned long long)c); return; }
+    }
+    atomicExch(&T.state[1], 1ull);
+}
+// One CTA per block with hits.  When every by-field of the block is a dict, const or absent column its key is a function of (bucket, dict ids):
+// a single-bucket block counts its rows per dict-id code in shared memory and inserts one representative per code (with no by-fields: one
+// insert of the block's count); a multi-bucket block merges runs of equal (bucket, code) inside each warp first.  Strings and typed columns
+// insert row by row.
+static __global__ void __launch_bounds__(256) k_hits_group(BatchView B, HitsQuery q, HitsView V, HitsTable T, const uint32_t* __restrict__ counts, const uint64_t* __restrict__ hit_offs,
+                                                            unsigned long long* __restrict__ stats) {
+    __shared__ uint32_t s_cnt[VL_HITS_CODES], s_rep[VL_HITS_CODES];
+    for (uint32_t b = blockIdx.x; b < B.nblocks; b += gridDim.x) {
+        const uint32_t n = counts[b];
+        if (n == 0) continue;
+        const uint64_t h0 = hit_offs[b];
+        bool agg = true;
+        uint32_t codes = 1, stride[VL_HITS_MAX_BY];
+        const uint8_t* ids[VL_HITS_MAX_BY];
+        for (uint32_t f = 0; f < q.nby; f++) {
+            stride[f] = codes; ids[f] = nullptr;
+            if (q.slot[f] < 0) continue;
+            const DevColumn& c = B.cols[(uint64_t)b * B.nfields + q.slot[f]];
+            if (c.kind != COL_VALUES) continue;
+            if (c.vt != VT_DICT) { agg = false; continue; }
+            const uint32_t width = c.dict_len ? c.dict_len : 1;
+            if (codes * width > VL_HITS_CODES) { agg = false; continue; }
+            ids[f] = B.arena + c.data_off;
+            codes *= width;
+        }
+        auto code_of = [&](uint32_t r) { uint32_t k = 0; for (uint32_t f = 0; f < q.nby; f++) if (ids[f]) k += ids[f][r] * stride[f]; return k; };
+        if (agg && !V.blk_multi[b]) {
+            const int64_t bucket = V.blk_bucket[b];
+            if (codes == 1) { if (threadIdx.x == 0) hits_insert(B, q, V, T, bucket, h0, b, V.hits[h0], n, stats); continue; }
+            for (uint32_t k = threadIdx.x; k < codes; k += blockDim.x) { s_cnt[k] = 0; s_rep[k] = 0xFFFFFFFFu; }
+            __syncthreads();
+            for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+                const uint32_t k = code_of(V.hits[h0 + i]);
+                if (k >= codes) { atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_DICT_INDEX); continue; }
+                atomicAdd(&s_cnt[k], 1u); atomicMin(&s_rep[k], i);
+            }
+            __syncthreads();
+            for (uint32_t k = threadIdx.x; k < codes; k += blockDim.x)
+                if (s_cnt[k]) hits_insert(B, q, V, T, bucket, h0 + s_rep[k], b, V.hits[h0 + s_rep[k]], s_cnt[k], stats);
+            __syncthreads();
+            continue;
+        }
+        const uint32_t lane = lane_id();
+        for (uint32_t base = 0; base < n; base += blockDim.x) {
+            const uint32_t i = base + threadIdx.x;
+            const int valid = i < n;
+            const uint32_t r = valid ? V.hits[h0 + i] : 0;
+            const int64_t bucket = valid ? hit_bucket(B, q, V, b, r) : 0;
+            const uint32_t k = valid && agg ? code_of(r) : 0;
+            const int64_t pb = __shfl_up_sync(0xffffffffu, bucket, 1);
+            const uint32_t pk = __shfl_up_sync(0xffffffffu, k, 1);
+            const int pv = __shfl_up_sync(0xffffffffu, valid, 1);
+            const int same_prev = agg && lane > 0 && valid && pv && pb == bucket && pk == k;
+            const uint32_t heads = __ballot_sync(0xffffffffu, valid && !same_prev);
+            int same_next = __shfl_down_sync(0xffffffffu, same_prev, 1);
+            if (lane == 31) same_next = 0;
+            if (valid && !same_next) {
+                const uint32_t head = 31 - __clz(heads & (0xffffffffu >> (31 - lane)));
+                hits_insert(B, q, V, T, bucket, h0 + i, b, r, lane - head + 1, stats);
+            }
+        }
+    }
+}
+// occupied slots -> groups: representative (row, block), bucket, count
+static __global__ void k_hits_emit(BatchView B, HitsQuery q, HitsView V, HitsTable T, uint32_t* __restrict__ rep_rows, uint32_t* __restrict__ rep_blocks, long long* __restrict__ buckets,
+                                   unsigned long long* __restrict__ out_counts) {
+    const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s > T.mask) return;
+    const unsigned long long tag = T.tags[s];
+    if (!tag) return;
+    const uint64_t rep = (tag & 0xFFFFFFFFull) - 1;
+    const uint64_t g = atomicAdd(&T.state[2], 1ull);
+    const uint32_t b = V.hit_block[rep], r = V.hits[rep];
+    rep_rows[g] = r; rep_blocks[g] = b; buckets[g] = hit_bucket(B, q, V, b, r); out_counts[g] = T.cnt[s];
 }
 
 }  // namespace vl

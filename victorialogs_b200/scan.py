@@ -61,6 +61,17 @@ class CStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+BUCKET_PLAIN, BUCKET_WEEK, BUCKET_MONTH, BUCKET_YEAR = 0, 1, 2, 3
+HITS_MAX_BY = 4
+GEN_TIMESTAMPS = 1 << 4                   # vlscan_gen_config.columns_mask bit: a timestamps column per generated block
+GEN_T0, GEN_STEP = 1700000000000000000, 1000000   # row i of a generated data set is at GEN_T0 + i * GEN_STEP nanoseconds
+
+
+class HitsQuery(C.Structure):
+    _fields_ = [("step", C.c_int64), ("offset", C.c_int64), ("calendar", C.c_uint32), ("nby", C.c_uint32),
+                ("by_names", C.POINTER(C.c_char_p)), ("by_name_lens", C.POINTER(C.c_size_t))]
+
+
 class GenConfig(C.Structure):
     _fields_ = [("seed", C.c_uint64), ("total_rows", C.c_uint64), ("rows_per_block", C.c_uint32), ("hot_block_permille", C.c_uint32),
                 ("hit_row_permille", C.c_uint32), ("columns_mask", C.c_uint32)]
@@ -71,7 +82,7 @@ EXPORTS = ["vlscan_device_count", "vlscan_ctx_create", "vlscan_ctx_free", "vlsca
            "vlscan_batch_upload", "vlscan_batch_free", "vlscan_batch_nblocks", "vlscan_batch_rows", "vlscan_batch_words", "vlscan_batch_device_bytes",
            "vlscan_batch_generate", "vlscan_batch_download", "vlscan_host_blocks_get", "vlscan_host_blocks_field", "vlscan_host_blocks_bytes",
            "vlscan_host_blocks_free", "vlscan_host_blocks_compress", "vlscan_zstd_decompress", "vlscan_zstd_inspect", "vlscan_zstd_walk_digest", "vlscan_part_open", "vlscan_part_free", "vlscan_part_header", "vlscan_part_nblocks", "vlscan_part_block_header", "vlscan_part_timestamps",
-           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch"]
+           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_truncate_timestamp", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch"]
 
 
 def lib_path():
@@ -100,6 +111,8 @@ def lib():
         for n in ("vlscan_ctx_free", "vlscan_program_free", "vlscan_batch_free", "vlscan_host_blocks_free"):
             getattr(L, n).argtypes = [C.c_void_p]
             getattr(L, n).restype = None
+        L.vlscan_truncate_timestamp.argtypes = [C.c_int64, C.c_int64, C.c_int64, C.c_uint32]
+        L.vlscan_truncate_timestamp.restype = C.c_int64
         L.vlscan_format_float64.argtypes = [C.c_uint64, C.c_char_p, C.c_size_t]
         L.vlscan_format_float64.restype = C.c_int
         _LIB = L
@@ -154,6 +167,19 @@ def format_float64(bits):
     if n < 0:
         raise ValueError(bits)
     return buf.raw[:n]
+
+
+def truncate_timestamp(ts, step, offset=0, calendar=BUCKET_PLAIN):
+    """The `_time` bucket of one timestamp (vlscan_truncate_timestamp: host build of the hits kernels' truncateTimestamp)."""
+    return lib().vlscan_truncate_timestamp(ts, step, offset, calendar)
+
+
+def hits_query(step, offset=0, calendar=BUCKET_PLAIN, by=()):
+    """-> (vlscan_hits_query, objects that must stay alive while it is used)"""
+    names = [_b(f) for f in by]
+    arr = (C.c_char_p * max(len(names), 1))(*names)
+    lens = (C.c_size_t * max(len(names), 1))(*[len(x) for x in names])
+    return HitsQuery(step, offset, calendar, len(names), arr, lens), (arr, lens)
 
 
 def parse_math_number(s):
@@ -723,6 +749,36 @@ class Ctx:
         n = int(hoffs[-1])
         raw = out.tobytes()
         return [raw[int(voffs[i]):int(voffs[i + 1])] for i in range(n)], hoffs
+
+    def hits_stats(self, step, offset=0, calendar=BUCKET_PLAIN, by=(), batch=None, info=None):
+        """`stats by (_time:step offset off, by...) count()` over the selected rows of the last scan (vlscan_hits_stats)
+        -> [(bucket, (key texts as bytes...), count)] sorted by bucket, then by the texts.  `info` (a dict) receives groups, key_bytes,
+        rows (selected) and blocks_decoded (blocks whose timestamps had to be decoded)."""
+        batch = batch or getattr(self, "_last", None)
+        q, keep = hits_query(step, offset, calendar, by)
+        nby = len(by)
+        cap_groups, cap_bytes = max(1, min(int(batch.rows) if batch else 0, 1 << 16)), 1 << 16
+        out_info = (C.c_uint64 * 4)()
+        for _ in range(2):
+            buckets = np.zeros(cap_groups, dtype=np.int64)
+            counts = np.zeros(cap_groups, dtype=np.uint64)
+            offs = np.zeros(cap_groups * nby + 1, dtype=np.uint64)
+            kb = np.zeros(max(cap_bytes, 1), dtype=np.uint8)
+            rc = lib().vlscan_hits_stats(self.h, C.byref(q), buckets.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p), C.c_uint64(cap_groups),
+                                         kb.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes), offs.ctypes.data_as(C.c_void_p), out_info)
+            if rc and (out_info[0] > cap_groups or out_info[1] > cap_bytes):
+                cap_groups, cap_bytes = max(cap_groups, out_info[0]), max(cap_bytes, out_info[1])
+                continue
+            self._check(rc)
+            break
+        if info is not None:
+            info.update(groups=out_info[0], key_bytes=out_info[1], rows=out_info[2], blocks_decoded=out_info[3])
+        raw = kb.tobytes()
+        out = []
+        for g in range(int(out_info[0])):
+            keys = tuple(raw[int(offs[g * nby + f]):int(offs[g * nby + f + 1])] for f in range(nby))
+            out.append((int(buckets[g]), keys, int(counts[g])))
+        return out
 
     def result_digest(self, block_lo, block_hi, key_base=0):
         """xor over blocks of XXH64(bitmap words) * (2 * (key_base + block) + 1) of the last scan, computed on the device (vlscan_result_digest)"""
