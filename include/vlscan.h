@@ -111,7 +111,10 @@ typedef struct vlscan_gen_config {
     uint32_t hit_row_permille;
     uint32_t columns_mask;       /* bit0 _msg, bit1 level, bit2 path, bit3 status; bit4 a timestamps column: row i of the data set at
                                     VLSCAN_GEN_T0 + i ms (MarshalTypeDeltaConst); bits 8..11: vocabulary focus for selectivity sweeps
-                                    (0 = a vocabulary row draws one of the 12 entries uniformly, k = always entry k - 1) */
+                                    (0 = a vocabulary row draws one of the 12 entries uniformly, k = always entry k - 1); bits 12..16,
+                                    only together with bit 4: k <= 16, S = 2^k blocks interleave in time: row i of block b at
+                                    VLSCAN_GEN_T0 + ((b / S) * S * rows_per_block + i * S + b % S) ms, still DeltaConst (k = 0: as bit 4
+                                    alone) */
 } vlscan_gen_config;
 #define VLSCAN_GEN_T0 1700000000000000000ll   /* 2023-11-14T22:13:20Z, nanoseconds */
 #define VLSCAN_GEN_STEP 1000000ll            /* 1 ms between consecutive rows */
@@ -344,6 +347,31 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
                       uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t out_info[4]);
 /* The bucket of one timestamp: host build of the routine the hits kernels run per row (truncateTimestamp above).  For tests. */
 int64_t vlscan_truncate_timestamp(int64_t ts, int64_t step, int64_t offset, uint32_t calendar);
+/* ---- the N newest selected rows: `/select/logsql/query?limit=N` (app/vlselect/logsql/logsql.go:932-948, 1005-1080 getLastNQueryResults) ---------
+ * Same preconditions as the gather calls: the result of the last vlscan_scan_resident of the ctx, whose batch must still be alive.  Every block
+ * with selected rows must have been staged with its timestamps.  The call leaves that result as it was: vlscan_fetch_results, the gather calls
+ * and vlscan_hits_stats return afterwards what they returned before it.
+ *   rows: the selected rows with _time >= min_timestamp, ordered by (timestamp, block index, row); the last min(limit, count) of them are
+ *     returned in that ascending order (getLastNRows after sortLogRows; among equal timestamps the later rows win, across blocks the higher
+ *     block index, so the result is deterministic).  A caller that merges batches passes the N-th newest timestamp it holds so far as
+ *     min_timestamp: the batch then returns only rows that can still enter the merged result (INTEGRATION.md §3d).
+ *   field_names: canonical names ("" = _msg); "_time" is rejected (it is out_timestamps).  The text of field f of returned row i is exactly what
+ *     vlscan_gather_values yields for that row: out_bytes[out_offsets[i * nfields + f], out_offsets[i * nfields + f + 1]) (out_offsets has
+ *     cap_rows * nfields + 1 entries).
+ * Output per row: out_timestamps[i], out_blocks[i] (block index in the batch), out_rows[i] (row in its block).
+ * out_info (may be NULL) = {rows returned, value bytes, selected rows, blocks whose timestamps were decoded}; it is filled also when the call fails
+ * because cap_rows or cap_bytes is too small (then nothing else is written).  Blocks are pruned by their headers: only blocks whose maximum
+ * timestamp reaches the weighted limit-th largest block minimum are looked at row by row, and blocks whose minimum equals their maximum are
+ * never decoded.  A block whose decoded timestamps contradict its header fails the call.  At most 2^32 - 2 selected rows per batch. */
+typedef struct vlscan_last_query {
+    uint64_t limit;                /* N >= 1                                                                                       */
+    int64_t min_timestamp;         /* rows older than this are not candidates (INT64_MIN = no floor)                               */
+    uint32_t nfields;              /* fields to return for each row                                                                */
+    const char* const* field_names;
+    const size_t* field_name_lens;
+} vlscan_last_query;
+int vlscan_last_rows(vlscan_ctx* ctx, const vlscan_last_query* q, int64_t* out_timestamps, uint32_t* out_blocks, uint32_t* out_rows, uint64_t cap_rows,
+                     uint8_t* out_bytes, uint64_t cap_bytes, uint64_t* out_offsets, uint64_t out_info[4]);
 /* Digest of the last scan's bitmaps of the blocks [block_lo, block_hi) of its batch, computed on the device: xor over the blocks of
  * XXH64(the block's bitmap words as little-endian bytes) * (2 * (key_base + block index) + 1).  The oracle reports the same quantity for its own
  * bitmaps, so a bench can check a billion-row scan against the CPU restatement on any block range without moving the bitmaps.  The batch of the

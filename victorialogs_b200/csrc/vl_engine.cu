@@ -833,7 +833,7 @@ void vlscan_ctx_free(vlscan_ctx* ctx) {
     for (auto& r : ctx->row_off8) r.release();
     for (auto& r : ctx->ready) r.release();
     ctx->zsrc.release(); ctx->zcols.release(); ctx->ztest.release(); ctx->ts_vals.release();
-    for (DevBuf* b : {&ctx->hit_block, &ctx->glens, &ctx->goffs, &ctx->gtiles, &ctx->gout, &ctx->gstat}) b->release();
+    for (DevBuf* b : {&ctx->hit_block, &ctx->glens, &ctx->goffs, &ctx->gtiles, &ctx->gout, &ctx->gstat, &ctx->hblk, &ctx->htab, &ctx->hgrp, &ctx->lcand}) b->release();
     zstd_dev_free(ctx->zdev);
     delete ctx->pool;
     if (ctx->pinned) cudaFreeHost(ctx->pinned);
@@ -1305,8 +1305,9 @@ static void check_gather_errors(vlscan_ctx* ctx) {
     VL_CUDA(cudaMemcpyAsync(h, ctx->gstat.p, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
     VL_CUDA(cudaStreamSynchronize(ctx->stream));
     static const char* const msg[] = {"", "cannot unmarshal strings: row lengths do not add up to the data length", "too big index for dict value", "unexpected length for binary representation of a number", "",
-                                      "unexpected uint64 block type", "the timestamps of a block with selected rows were not handed over", "cannot unmarshal timestamps"};
-    if (h[ST_ERROR]) throw BadInput(msg[std::min<unsigned long long>(h[ST_ERROR], 7)]);
+                                      "unexpected uint64 block type", "the timestamps of a block with selected rows were not handed over", "cannot unmarshal timestamps", "",
+                                      "the decoded timestamps of a block contradict the minimum / maximum of its header"};
+    if (h[ST_ERROR]) throw BadInput(msg[std::min<unsigned long long>(h[ST_ERROR], 9)]);
 }
 
 int vlscan_gather_timestamps(vlscan_ctx* ctx, int64_t* out_timestamps, uint64_t cap, uint64_t* out_hit_offsets) {
@@ -1334,13 +1335,14 @@ static int field_slot(const vlscan_batch* b, const std::string& name) {
     for (uint32_t s = 0; s < b->nfields; s++) if (b->field_names[s] == name) return (int)s;
     return -1;
 }
-// row offsets of the strings blocks with hits in column `slot` (kept from the scan where it already computed them)
-static const uint32_t* hit_row_offsets(vlscan_ctx* ctx, int slot) {
+// row offsets of the strings blocks with hits in column `slot` (kept from the scan where it already computed them); `with_rows` (default: the
+// scan's counts) != 0 marks the blocks whose offsets are needed
+static const uint32_t* hit_row_offsets(vlscan_ctx* ctx, int slot, const uint32_t* with_rows = nullptr) {
     if (slot < 0) return nullptr;
     BatchView B = ctx->last_batch->view();
     uint32_t* wc = ctx->work_count.as<uint32_t>();
     VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
-    k_hit_blocks_list<<<cdiv(B.nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), slot, 0, ctx->lens_blocks.as<uint32_t>(), wc); launch_check(ctx);
+    k_hit_blocks_list<<<cdiv(B.nblocks, 256), 256, 0, ctx->stream>>>(B, with_rows ? with_rows : ctx->counts.as<uint32_t>(), slot, 0, ctx->lens_blocks.as<uint32_t>(), wc); launch_check(ctx);
     uint8_t* ready = ctx->ready[slot].as<uint8_t>();
     if (!ctx->ready_cleared[slot]) { VL_CUDA(cudaMemsetAsync(ready, 0, B.nblocks, ctx->stream)); ctx->ready_cleared[slot] = 1; }
     k_lens_offsets<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(B, slot, ctx->lens_blocks.as<uint32_t>(), wc, ctx->row_off8[slot].as<uint32_t>(), ready, ctx->gstat.as<unsigned long long>()); launch_check(ctx);
@@ -1492,6 +1494,151 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
                 const std::string_view t = text(f, g);
                 memcpy(out_key_bytes + o, t.data(), t.size()); o += t.size();
                 out_key_offsets[i * q->nby + f + 1] = o;
+            }
+        }
+    });
+    if (out_info) memcpy(out_info, info, sizeof info);
+    return rc;
+}
+
+// the limit-th largest of the n int64 keys (weights: NULL = 1 each) into the radix state st (RS_COUNT words + VL_RADIX_PASSES histograms), on
+// the stream, with no host round trip
+static void radix_select(vlscan_ctx* ctx, const long long* keys, const uint32_t* weights, uint64_t n, uint64_t limit, unsigned long long* st) {
+    VL_CUDA(cudaMemsetAsync(st, 0, (RS_COUNT + VL_RADIX_PASSES * 256) * 8, ctx->stream));
+    const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(cdiv(n, 256), (uint64_t)ctx->sm_count * 8));
+    for (int p = 0; p < VL_RADIX_PASSES; p++) {
+        const int shift = 64 - 8 * (p + 1);
+        unsigned long long* hist = st + RS_COUNT + p * 256;
+        k_radix_hist<<<grid, 256, 0, ctx->stream>>>(keys, weights, n, st, shift, hist); launch_check(ctx);
+        k_radix_pick<<<1, 32, 0, ctx->stream>>>(hist, shift, limit, st); launch_check(ctx);
+    }
+}
+
+int vlscan_last_rows(vlscan_ctx* ctx, const vlscan_last_query* q, int64_t* out_timestamps, uint32_t* out_blocks, uint32_t* out_rows, uint64_t cap_rows,
+                     uint8_t* out_bytes, uint64_t cap_bytes, uint64_t* out_offsets, uint64_t out_info[4]) {
+    uint64_t info[4] = {0, 0, 0, 0};   // rows returned, value bytes, selected rows, blocks whose timestamps were decoded
+    const int rc = guarded(ctx, [&] {
+        if (!q) throw BadInput("no last-rows query");
+        if (q->limit == 0) throw BadInput("the limit of vlscan_last_rows must be at least 1");
+        if (q->nfields && (!q->field_names || !q->field_name_lens)) throw BadInput("vlscan_last_rows: field names missing");
+        std::vector<std::string> names;
+        for (uint32_t f = 0; f < q->nfields; f++) {
+            std::string n(q->field_names[f], q->field_name_lens[f]);
+            if (n.empty()) n = "_msg";   // getCanonicalColumnName
+            if (n == "_time") throw BadInput("`_time` cannot be a field of vlscan_last_rows: it is returned in out_timestamps");
+            names.push_back(n);
+        }
+        if (!ctx) throw BadInput("vlscan_last_rows needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
+        if (!ctx->has_result) throw BadInput("no scan result on this ctx");
+        VL_CUDA(cudaSetDevice(ctx->device));
+        const vlscan_batch* b = ctx->last_batch;
+        BatchView B = b->view();
+        const uint64_t nb = b->nblocks, limit = q->limit;
+        const long long floor_ts = q->min_timestamp;
+        const uint32_t* counts = ctx->counts.as<uint32_t>();
+        ctx->gstat.ensure(ST_COUNT * 8);
+        VL_CUDA(cudaMemsetAsync(ctx->gstat.p, 0, ST_COUNT * 8, ctx->stream));
+        unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
+        ctx->hblk.ensure(nb * 28 + 64);
+        long long* blk_key = ctx->hblk.as<long long>();
+        uint64_t* cand_offs = (uint64_t*)(blk_key + nb);
+        uint32_t* blk_w = (uint32_t*)(cand_offs + nb + 1); uint32_t* cand_rows = blk_w + nb; uint32_t* blk_mark = cand_rows + nb;
+        const size_t st_words = RS_COUNT + VL_RADIX_PASSES * 256;
+        ctx->htab.ensure(2 * st_words * 8);
+        unsigned long long* st_blk = ctx->htab.as<unsigned long long>(); unsigned long long* st_row = st_blk + st_words;
+        ctx->hit_offs.ensure((nb + 1) * 8); ctx->lens_blocks2.ensure(nb * 4 + 16); ctx->row_blocks.ensure(nb * 4 + 16);
+        k_scan_counts<<<1, 1024, 0, ctx->stream>>>(counts, (uint32_t)nb, ctx->hit_offs.as<uint64_t>()); launch_check(ctx);
+        // (1) the block threshold T_lo, from the headers alone
+        if (nb) { k_last_block_keys<<<cdiv(nb, 256), 256, 0, ctx->stream>>>(B, counts, floor_ts, blk_key, blk_w, gstat); launch_check(ctx); }
+        radix_select(ctx, blk_key, blk_w, nb, limit, st_blk);
+        // (2) the candidate blocks, the timestamps of those that are not flat, and the count of their selected rows >= T_lo
+        uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* cand = ctx->lens_blocks2.as<uint32_t>(); uint32_t* decode = ctx->row_blocks.as<uint32_t>();
+        VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
+        VL_CUDA(cudaMemsetAsync(cand_rows, 0, nb * 8, ctx->stream));   // cand_rows and blk_mark
+        if (nb) { k_last_candidates<<<cdiv(nb, 256), 256, 0, ctx->stream>>>(B, counts, floor_ts, st_blk, cand, decode, wc); launch_check(ctx); }
+        ctx->ts_vals.ensure(b->nwords * 64 * 8);
+        unsigned long long* ts_vals = ctx->ts_vals.as<unsigned long long>();
+        k_ts_decode_list<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(B, decode, wc, ts_vals, gstat); launch_check(ctx);
+        const unsigned row_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(nb, (uint64_t)ctx->sm_count * 8));
+        k_last_rows<<<row_grid, 256, 0, ctx->stream>>>(B, ctx->regs[0].as<uint64_t>(), cand, wc, ts_vals, floor_ts, st_blk, 0, cand_rows, nullptr, nullptr, nullptr, nullptr, gstat);
+        launch_check(ctx);
+        k_scan_counts<<<1, 1024, 0, ctx->stream>>>(cand_rows, (uint32_t)nb, cand_offs); launch_check(ctx);
+        uint64_t selected = 0, M = 0; unsigned long long blk_short = 0; uint32_t decoded = 0;
+        VL_CUDA(cudaMemcpyAsync(&selected, ctx->hit_offs.as<uint64_t>() + nb, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaMemcpyAsync(&M, cand_offs + nb, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaMemcpyAsync(&blk_short, st_blk + RS_SHORT, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaMemcpyAsync(&decoded, wc + WC_ROW, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        check_gather_errors(ctx);   // synchronises
+        info[2] = selected; info[3] = decoded;
+        if (selected >= 0xFFFFFFFFull) throw BadInput("more than 2^32 - 2 selected rows in one batch");
+        // the block weights promise `limit` rows >= T_lo; fewer means a block's timestamps disagree with its header
+        if (!blk_short && M < limit) throw BadInput("the decoded timestamps of a block contradict the minimum / maximum of its header");
+        const uint64_t n = std::min<uint64_t>(limit, M);
+        std::vector<int64_t> hts(n); std::vector<uint32_t> hb(n), hr(n);
+        uint32_t* sel_blk = nullptr; uint32_t* sel_row = nullptr;
+        if (n) {
+            // the candidates in (block, row) order, then (3) the exact top N: T_N, every row above it and the last ties
+            ctx->lcand.ensure(M * 16 + 64);
+            long long* cts = ctx->lcand.as<long long>(); uint32_t* cblk = (uint32_t*)(cts + M); uint32_t* crow = cblk + M;
+            k_last_rows<<<row_grid, 256, 0, ctx->stream>>>(B, ctx->regs[0].as<uint64_t>(), cand, wc, ts_vals, floor_ts, st_blk, 1, nullptr, cand_offs, cts, cblk, crow, gstat);
+            launch_check(ctx);
+            radix_select(ctx, cts, nullptr, M, limit, st_row);
+            const uint64_t ntiles = cdiv(M, VL_SCAN_TILE);
+            ctx->glens.ensure(M * 4); ctx->goffs.ensure((M + 1) * 8); ctx->gtiles.ensure((ntiles + 1) * 8);
+            k_last_ties<<<cdiv(M, 256), 256, 0, ctx->stream>>>(cts, M, st_row, ctx->glens.as<uint32_t>()); launch_check(ctx);
+            k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(ctx->glens.as<uint32_t>(), M, ctx->gtiles.as<unsigned long long>(), nullptr, 0); launch_check(ctx);
+            k_scan_tile_sums<<<1, 1024, 0, ctx->stream>>>(ctx->gtiles.as<unsigned long long>(), ntiles, ctx->goffs.as<unsigned long long>() + M); launch_check(ctx);
+            k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(ctx->glens.as<uint32_t>(), M, ctx->gtiles.as<unsigned long long>(), ctx->goffs.as<unsigned long long>(), 1); launch_check(ctx);
+            ctx->hgrp.ensure(n * 16 + 64);
+            long long* sel_ts = ctx->hgrp.as<long long>(); unsigned long long* sel_n = (unsigned long long*)(sel_ts + n);
+            sel_blk = (uint32_t*)(sel_n + 1); sel_row = sel_blk + n;
+            VL_CUDA(cudaMemsetAsync(sel_n, 0, 8, ctx->stream));
+            k_last_choose<<<cdiv(M, 256), 256, 0, ctx->stream>>>(cts, cblk, crow, M, st_row, ctx->goffs.as<uint64_t>(), sel_ts, sel_blk, sel_row, sel_n, blk_mark); launch_check(ctx);
+            uint64_t chosen = 0;
+            VL_CUDA(cudaMemcpyAsync(&chosen, sel_n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(hts.data(), sel_ts, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(hb.data(), sel_blk, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(hr.data(), sel_row, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaStreamSynchronize(ctx->stream));
+            if (chosen != n) throw BadInput("internal: the top-N selection chose " + std::to_string(chosen) + " rows instead of " + std::to_string(n));
+        }
+        // (4) the texts of the chosen rows only
+        std::vector<std::vector<uint64_t>> toffs(q->nfields); std::vector<std::vector<uint8_t>> tbytes(q->nfields);
+        uint64_t value_bytes = 0;
+        for (uint32_t f = 0; f < q->nfields && n; f++) {
+            const int slot = field_slot(b, names[f]);
+            const uint32_t* ro = hit_row_offsets(ctx, slot, blk_mark);
+            const uint64_t total = text_offsets(ctx, slot, ro, sel_row, sel_blk, n);
+            value_bytes += total;
+            toffs[f].resize(n + 1); tbytes[f].resize(total);
+            text_bytes(ctx, slot, ro, sel_row, sel_blk, n, total);
+            VL_CUDA(cudaMemcpyAsync(toffs[f].data(), ctx->goffs.p, (n + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+            if (total) VL_CUDA(cudaMemcpyAsync(tbytes[f].data(), ctx->gout.p, total, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaStreamSynchronize(ctx->stream));
+        }
+        check_gather_errors(ctx);
+        info[0] = n; info[1] = value_bytes;
+        if (n > cap_rows) throw BadInput("rows buffer too small (the needed size is reported)");
+        if (value_bytes > cap_bytes) throw BadInput("value bytes buffer too small (the needed size is reported)");
+        if ((n && (!out_timestamps || !out_blocks || !out_rows)) || (q->nfields && !out_offsets) || (value_bytes && !out_bytes)) throw BadInput("last-rows output buffer missing");
+        // ascending (timestamp, block, row): getLastNRows' order
+        std::vector<uint64_t> order(n);
+        for (uint64_t i = 0; i < n; i++) order[i] = i;
+        std::sort(order.begin(), order.end(), [&](uint64_t x, uint64_t y) {
+            if (hts[x] != hts[y]) return hts[x] < hts[y];
+            if (hb[x] != hb[y]) return hb[x] < hb[y];
+            return hr[x] < hr[y];
+        });
+        if (out_offsets) out_offsets[0] = 0;
+        uint64_t o = 0;
+        for (uint64_t i = 0; i < n; i++) {
+            const uint64_t k = order[i];
+            out_timestamps[i] = hts[k]; out_blocks[i] = hb[k]; out_rows[i] = hr[k];
+            for (uint32_t f = 0; f < q->nfields; f++) {
+                const uint64_t a = toffs[f][k], len = toffs[f][k + 1] - a;
+                if (len) memcpy(out_bytes + o, tbytes[f].data() + a, len);
+                o += len;
+                out_offsets[i * q->nfields + f + 1] = o;
             }
         }
     });

@@ -92,7 +92,9 @@ struct vlscan_ctx {
     std::vector<char> ready_cleared;
     vl::DevBuf hit_block, glens, goffs, gtiles, gout, gstat;   // hit materialisation (vlscan_gather_*): block of each hit, value lengths / offsets, output staging, error slot
     vl::DevBuf ts_vals;                    // decoded timestamps / running sums, 8 bytes per row of the batch (k_time_match, gather)
-    vl::DevBuf hblk, htab, hgrp;           // vlscan_hits_stats: per-block bucket + multi-bucket flag, the group table (tags, counts, state), the emitted groups
+    vl::DevBuf hblk, htab, hgrp;           // vlscan_hits_stats: per-block bucket + multi-bucket flag, the group table (tags, counts, state), the emitted groups;
+                                           // vlscan_last_rows: per-block keys / weights / counts / offsets, the radix select states, the chosen rows
+    vl::DevBuf lcand;                      // vlscan_last_rows: the candidate rows (timestamp, block, row)
     vl::DevBuf need;                       // bloom-first probe pass: one byte per (block, field), set when the column's values must be staged
     const void* bf_prog = nullptr; int bf_skip = 0;   // adaptive bloom-first: after a probe that pruned next to nothing, the next calls with the same program stage everything at once
     vl::DevBuf zsrc, zcols, ztest;         // compressed staging of on-disk values blocks; their column list; test output

@@ -9,7 +9,9 @@
 //   * `status`: uint16 column, big-endian values + min/max (values_encoder.go:1168-1222),
 //   * bloom filters: 16 bits per unique token hash, 6 probes, big-endian u64 words (bloomfilter.go:83-121).
 //   * timestamps (columns_mask bit 4): row i of the data set at VLSCAN_GEN_T0 + i * VLSCAN_GEN_STEP, a constant delta, so every block is
-//     MarshalTypeDeltaConst: the varint of the delta and nothing else (vm/lib/encoding/encoding.go:119-130).
+//     MarshalTypeDeltaConst: the varint of the delta and nothing else (vm/lib/encoding/encoding.go:119-130).  Bits 12..16 = k (with bit 4
+//     only) interleave S = 2^k blocks: row i of block b at VLSCAN_GEN_T0 + ((b / S) * S * rows_per_block + i * S + b % S) * VLSCAN_GEN_STEP, so
+//     the S blocks of a group overlap in time; still DeltaConst, with delta S * VLSCAN_GEN_STEP.  k = 0 is the plain series above.
 // tests/test_gpu_gen.py checks the output byte-for-byte against the CPU oracle's restatement of that writer path.
 //
 // Supported envelope (anything else is refused with an error instead of silently diverging from the writer):
@@ -247,7 +249,11 @@ extern "C" int vlscan_batch_generate(vlscan_ctx* ctx, const vlscan_gen_config* c
         int slot_of[4]; bt->nfields = 0;
         for (int k = 0; k < 4; k++) { slot_of[k] = -1; if (c.columns_mask >> k & 1) { slot_of[k] = (int)bt->nfields++; bt->field_names.push_back(names[k]); } }
         if (!bt->nfields) throw BadInput("generator: empty columns_mask");
-        if (((c.columns_mask >> 8) & 15) > 12 || (c.columns_mask >> 12)) throw BadInput("generator: bits 8..11 of columns_mask select a vocabulary entry 1..12, higher bits must be zero");
+        if (((c.columns_mask >> 8) & 15) > 12 || (c.columns_mask >> 17) || ((c.columns_mask >> 12) && !(c.columns_mask & 16)))
+            throw BadInput("generator: bits 8..11 of columns_mask select a vocabulary entry 1..12, bits 12..16 (interleaved timestamp streams) need bit 4, higher bits must be zero");
+        const uint32_t ts_k = (c.columns_mask >> 12) & 31;
+        if (ts_k > 16) throw BadInput("generator: at most 2^16 interleaved timestamp streams (bits 12..16 of columns_mask)");
+        const uint64_t ts_streams = 1ull << ts_k;
         // pass A
         uint32_t cap = 1; while (cap < c.rows_per_block * 40u) cap <<= 1;   // <= ~26 tokens per _msg row
         int grid = std::min<int>(std::max<uint32_t>(nb, 1), ctx->sm_count * 2);
@@ -268,7 +274,7 @@ extern "C" int vlscan_batch_generate(vlscan_ctx* ctx, const vlscan_gen_config* c
         std::vector<DevTimestamps> tsv((c.columns_mask & 16) ? nb : 0);
         if (!tsv.empty()) memset(tsv.data(), 0, tsv.size() * sizeof(DevTimestamps));
         std::vector<uint8_t> ts_varint;
-        for (uint64_t u = (uint64_t)VLSCAN_GEN_STEP << 1; ; u >>= 7) { if (u < 0x80) { ts_varint.push_back((uint8_t)u); break; } ts_varint.push_back((uint8_t)(u | 0x80)); }
+        for (uint64_t u = (ts_streams * VLSCAN_GEN_STEP) << 1; ; u >>= 7) { if (u < 0x80) { ts_varint.push_back((uint8_t)u); break; } ts_varint.push_back((uint8_t)(u | 0x80)); }
         for (uint32_t j = 0; j < nb; j++) {
             const GenInfo& gi = info[j]; GenPlan& pl = plans[j]; uint32_t R = rows[j];
             if (gi.overflow) throw BadInput("generator: token set overflow");
@@ -307,8 +313,9 @@ extern "C" int vlscan_batch_generate(vlscan_ctx* ctx, const vlscan_gen_config* c
             }
             if (c.columns_mask & 16) {   // encoding.MarshalVarInt64(delta): zig-zag, then unsigned varint
                 DevTimestamps& t = tsv[j];
-                const uint64_t first = (uint64_t)VLSCAN_GEN_T0 + ((block_lo + j) * c.rows_per_block) * (uint64_t)VLSCAN_GEN_STEP;
-                t.first = (int64_t)first; t.max = (int64_t)(first + (uint64_t)(R - 1) * VLSCAN_GEN_STEP);
+                const uint64_t gb = block_lo + j;
+                const uint64_t first = (uint64_t)VLSCAN_GEN_T0 + ((gb / ts_streams) * ts_streams * c.rows_per_block + gb % ts_streams) * (uint64_t)VLSCAN_GEN_STEP;
+                t.first = (int64_t)first; t.max = (int64_t)(first + (uint64_t)(R - 1) * ts_streams * VLSCAN_GEN_STEP);
                 t.mt = MT_DELTA_CONST; t.len = (uint32_t)ts_varint.size(); t.off = arena_reserve(cursor, ts_varint.size());
             }
             if (slot_of[3] >= 0) {

@@ -17,7 +17,8 @@ struct DevProgram {
 
 // stats slots (device u64 array)
 enum { ST_VALUES_BYTES = 0, ST_BLOOM_BYTES, ST_COLUMNS_READ, ST_BITMAP_BYTES, ST_ROWS_MATCHED, ST_BLOCKS_MATCHED, ST_ERROR, ST_SCAN_BYTES, ST_COUNT };
-enum { ERR_NONE = 0, ERR_LENS_MISMATCH = 1, ERR_DICT_INDEX = 2, ERR_BAD_WIDTH = 3, ERR_UNSUPPORTED_FLOAT_TOSTRING = 4, ERR_BAD_LENS_TYPE = 5, ERR_NO_TIMESTAMPS = 6, ERR_BAD_TIMESTAMPS = 7, ERR_VALUES_ABSENT = 8 };
+enum { ERR_NONE = 0, ERR_LENS_MISMATCH = 1, ERR_DICT_INDEX = 2, ERR_BAD_WIDTH = 3, ERR_UNSUPPORTED_FLOAT_TOSTRING = 4, ERR_BAD_LENS_TYPE = 5, ERR_NO_TIMESTAMPS = 6, ERR_BAD_TIMESTAMPS = 7, ERR_VALUES_ABSENT = 8,
+       ERR_TS_HEADER = 9 };   // decoded timestamps outside the [min, max] of their block header (k_last_rows)
 
 struct BatchView {
     const uint8_t* arena;         // values payloads: lens items, data, encoded timestamps (lens_off, data_off, DevTimestamps.off)
@@ -1738,6 +1739,154 @@ static __global__ void k_hits_emit(BatchView B, HitsQuery q, HitsView V, HitsTab
     const uint64_t g = atomicAdd(&T.state[2], 1ull);
     const uint32_t b = V.hit_block[rep], r = V.hits[rep];
     rep_rows[g] = r; rep_blocks[g] = b; buckets[g] = hit_bucket(B, q, V, b, r); out_counts[g] = T.cnt[s];
+}
+
+// ---- the N newest selected rows: `/select/logsql/query?limit=N` (app/vlselect/logsql/logsql.go:1005-1080 getLastNQueryResults) ----------------
+// Timestamps inside a block never decrease (the writer refuses anything else, lib/logstorage/block.go:182,346), so every selected row of block b
+// lies in [min_b, max_b] of its header.  A weighted radix select over the minimums of the blocks with hits at or above the floor (weight: their
+// selected rows) gives T_lo, the limit-th largest: at least `limit` selected rows are >= T_lo, so only blocks with max_b >= T_lo can hold a
+// returned row, and every other block gets no per-row work.  The selected rows >= T_lo of those blocks are compacted in (block, row) order; the
+// same radix select over their timestamps (weight 1) gives T_N, the limit-th largest.  Rows above T_N are in; of the rows equal to T_N the last
+// ones in (block, row) order (a prefix count over the ties), which is getLastNRows after a stable sort by _time.
+// Radix select: int64 keys with the sign bit flipped (unsigned order = signed order), VL_RADIX_PASSES passes of 8 bits from the top.  The state
+// (RS_*) stays on the device, so the passes need no host round trip: after the last pass RS_PREFIX is the flipped limit-th largest key and RS_K
+// how many keys equal to it are needed; RS_SHORT = the weights add up to less than the limit.
+enum { RS_PREFIX = 0, RS_MASK = 1, RS_K = 2, RS_SHORT = 3, RS_COUNT = 4 };
+#define VL_RADIX_PASSES 8
+#define VL_SIGN64 0x8000000000000000ull
+static __device__ __forceinline__ long long radix_key(const unsigned long long* st) { return (long long)(st[RS_PREFIX] ^ VL_SIGN64); }
+// weighted histogram of the next digit of the keys that match the prefix chosen so far (weights == NULL: every key weighs 1)
+static __global__ void __launch_bounds__(256) k_radix_hist(const long long* __restrict__ keys, const uint32_t* __restrict__ weights, uint64_t n, const unsigned long long* __restrict__ st,
+                                                            int shift, unsigned long long* __restrict__ hist) {
+    __shared__ unsigned long long s_h[256];
+    s_h[threadIdx.x] = 0;
+    __syncthreads();
+    if (!st[RS_SHORT]) {
+        const unsigned long long prefix = st[RS_PREFIX], mask = st[RS_MASK];
+        const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+        for (uint64_t base = (uint64_t)blockIdx.x * blockDim.x; base < n; base += stride) {   // warp-uniform trip count: the match below takes every lane
+            const uint64_t i = base + threadIdx.x;
+            uint32_t w = 0, d = 0;
+            if (i < n) {
+                const unsigned long long u = (unsigned long long)keys[i] ^ VL_SIGN64;
+                w = (u & mask) != prefix ? 0u : weights ? weights[i] : 1u;
+                d = (uint32_t)(u >> shift) & 255u;
+            }
+            if (weights) {   // block minimums: few keys, spread out
+                if (w) atomicAdd(&s_h[d], (unsigned long long)w);
+            } else {         // row timestamps share their high digits: one shared atomic per group of equal digits in the warp
+                const uint32_t peers = __match_any_sync(0xffffffffu, w ? d : 256u);
+                if (w && lane_id() == (uint32_t)(__ffs(peers) - 1)) atomicAdd(&s_h[d], (unsigned long long)__popc(peers));
+            }
+        }
+    }
+    __syncthreads();
+    if (s_h[threadIdx.x]) atomicAdd(&hist[threadIdx.x], s_h[threadIdx.x]);
+}
+// the digit of this pass: the largest d whose keys, with those of the digits above it, reach the limit
+static __global__ void k_radix_pick(const unsigned long long* __restrict__ hist, int shift, unsigned long long limit, unsigned long long* __restrict__ st) {
+    if (threadIdx.x != 0 || st[RS_SHORT]) return;
+    unsigned long long k = st[RS_K];
+    if (shift == 64 - 8) {
+        unsigned long long total = 0;
+        for (int d = 0; d < 256; d++) total += hist[d];
+        if (total < limit) { st[RS_SHORT] = 1; return; }
+        k = limit;
+    }
+    unsigned long long above = 0;
+    int d = 255;
+    for (; d > 0; d--) {
+        if (above + hist[d] >= k) break;
+        above += hist[d];
+    }
+    st[RS_PREFIX] |= (unsigned long long)d << shift; st[RS_MASK] |= 0xFFull << shift; st[RS_K] = k - above;
+}
+// the key of the block threshold: the header minimum of a block with hits, weighted by its selected rows when it is at or above the floor
+static __global__ void k_last_block_keys(BatchView B, const uint32_t* __restrict__ counts, long long floor_ts, long long* __restrict__ keys, uint32_t* __restrict__ weights,
+                                         unsigned long long* __restrict__ stats) {
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B.nblocks) return;
+    uint32_t w = counts[b];
+    long long key = 0;
+    if (w) {
+        if (!B.ts || B.ts[b].mt == 0) { atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_NO_TIMESTAMPS); w = 0; }
+        else { key = B.ts[b].first; if (key < floor_ts) w = 0; }
+    }
+    keys[b] = key; weights[b] = w;
+}
+// T_lo = the block threshold, or the floor when the weights add up to less than the limit.  Candidate blocks (blocks with hits and max_b >= T_lo)
+// go into cand; those whose minimum and maximum differ also into the decode list (WC_ROW; a flat block's rows all carry its minimum).
+static __device__ __forceinline__ long long last_threshold(const unsigned long long* st, long long floor_ts) { return st[RS_SHORT] ? floor_ts : radix_key(st); }
+static __global__ void k_last_candidates(BatchView B, const uint32_t* __restrict__ counts, long long floor_ts, const unsigned long long* __restrict__ st, uint32_t* __restrict__ cand,
+                                         uint32_t* __restrict__ decode, uint32_t* __restrict__ work_count) {
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B.nblocks || counts[b] == 0 || !B.ts || B.ts[b].mt == 0) return;
+    const DevTimestamps& t = B.ts[b];
+    if (t.max < last_threshold(st, floor_ts)) return;
+    cand[atomicAdd(&work_count[WC_LENS2], 1u)] = b;
+    if (t.first != t.max) decode[atomicAdd(&work_count[WC_ROW], 1u)] = b;
+}
+// One CTA per candidate block: its selected rows with ts >= T_lo.  pass 0: their number -> cand_rows[b]; pass 1: (ts, block, row) at offs[b] + rank,
+// rows ascending.  A decoded timestamp outside the block's header range is reported (ERR_TS_HEADER).
+static __global__ void __launch_bounds__(256) k_last_rows(BatchView B, const uint64_t* __restrict__ reg, const uint32_t* __restrict__ cand, const uint32_t* __restrict__ work_count,
+                                                           const unsigned long long* __restrict__ ts_vals, long long floor_ts, const unsigned long long* __restrict__ st, int pass,
+                                                           uint32_t* __restrict__ cand_rows, const uint64_t* __restrict__ offs, long long* __restrict__ out_ts, uint32_t* __restrict__ out_blk,
+                                                           uint32_t* __restrict__ out_row, unsigned long long* __restrict__ stats) {
+    __shared__ uint32_t s_warp[8];
+    const uint32_t nwork = work_count[WC_LENS2];
+    const long long lo = last_threshold(st, floor_ts);
+    const uint32_t lane = lane_id(), wid = threadIdx.x >> 5;
+    for (uint32_t j = blockIdx.x; j < nwork; j += gridDim.x) {
+        const uint32_t b = cand[j], R = B.blk_rows[b];
+        const uint64_t w0 = B.blk_word_off[b];
+        const long long mn = B.ts[b].first, mx = B.ts[b].max;
+        const unsigned long long* vals = ts_vals + w0 * 64;
+        uint64_t o = pass ? offs[b] : 0;
+        bool bad = false;
+        for (uint32_t base = 0; base < R; base += blockDim.x) {
+            const uint32_t r = base + threadIdx.x;
+            long long t = mn;
+            bool f = false;
+            if (r < R) {
+                if (mn != mx) { t = (long long)vals[r]; bad |= t < mn || t > mx; }
+                f = (reg[w0 + (r >> 6)] >> (r & 63) & 1) && t >= lo;
+            }
+            const uint32_t m = __ballot_sync(0xffffffffu, f);
+            if (lane == 0) s_warp[wid] = __popc(m);
+            __syncthreads();
+            uint32_t pre = 0, tot = 0;
+            for (uint32_t k = 0; k < (blockDim.x >> 5); k++) { const uint32_t c = s_warp[k]; pre += k < wid ? c : 0; tot += c; }
+            if (pass && f) {
+                const uint64_t p = o + pre + __popc(m & ((1u << lane) - 1));
+                out_ts[p] = t; out_blk[p] = b; out_row[p] = r;
+            }
+            o += tot;
+            __syncthreads();
+        }
+        if (bad) atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_TS_HEADER);
+        if (pass == 0 && threadIdx.x == 0) cand_rows[b] = (uint32_t)o;
+    }
+}
+// eq[i] = candidate i carries T_N (the ties whose prefix count decides which of them stay)
+static __global__ void k_last_ties(const long long* __restrict__ cts, uint64_t n, const unsigned long long* __restrict__ st, uint32_t* __restrict__ eq) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) eq[i] = !st[RS_SHORT] && cts[i] == radix_key(st);
+}
+// the chosen candidates: ts > T_N, or ts == T_N among the last RS_K ties (eq_offs: exclusive prefix count of the ties, eq_offs[n] = all of them);
+// every candidate when there are no more than the limit.  Output order is arbitrary (the host sorts the <= limit rows); blk_mark[b] = 1 for their blocks.
+static __global__ void k_last_choose(const long long* __restrict__ cts, const uint32_t* __restrict__ cblk, const uint32_t* __restrict__ crow, uint64_t n, const unsigned long long* __restrict__ st,
+                                     const uint64_t* __restrict__ eq_offs, long long* __restrict__ out_ts, uint32_t* __restrict__ out_blk, uint32_t* __restrict__ out_row,
+                                     unsigned long long* __restrict__ out_n, uint32_t* __restrict__ blk_mark) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const long long t = cts[i];
+    if (!st[RS_SHORT]) {
+        const long long tn = radix_key(st);
+        if (t < tn || (t == tn && eq_offs[i] < eq_offs[n] - st[RS_K])) return;
+    }
+    const unsigned long long p = atomicAdd(out_n, 1ull);
+    out_ts[p] = t; out_blk[p] = cblk[i]; out_row[p] = crow[i];
+    blk_mark[cblk[i]] = 1;
 }
 
 }  // namespace vl

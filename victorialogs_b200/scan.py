@@ -65,11 +65,23 @@ BUCKET_PLAIN, BUCKET_WEEK, BUCKET_MONTH, BUCKET_YEAR = 0, 1, 2, 3
 HITS_MAX_BY = 4
 GEN_TIMESTAMPS = 1 << 4                   # vlscan_gen_config.columns_mask bit: a timestamps column per generated block
 GEN_T0, GEN_STEP = 1700000000000000000, 1000000   # row i of a generated data set is at GEN_T0 + i * GEN_STEP nanoseconds
+GEN_STREAMS_SHIFT = 12                    # columns_mask bits 12..16 = k (with GEN_TIMESTAMPS only): 2^k generated blocks interleave in time
+I64_MIN = -(1 << 63)
+
+
+def gen_streams(k):
+    """columns_mask bits that interleave 2^k generated blocks in time (row i of block b at GEN_T0 + ((b // S) * S * R + i * S + b % S) * GEN_STEP)"""
+    return k << GEN_STREAMS_SHIFT
 
 
 class HitsQuery(C.Structure):
     _fields_ = [("step", C.c_int64), ("offset", C.c_int64), ("calendar", C.c_uint32), ("nby", C.c_uint32),
                 ("by_names", C.POINTER(C.c_char_p)), ("by_name_lens", C.POINTER(C.c_size_t))]
+
+
+class LastQuery(C.Structure):
+    _fields_ = [("limit", C.c_uint64), ("min_timestamp", C.c_int64), ("nfields", C.c_uint32),
+                ("field_names", C.POINTER(C.c_char_p)), ("field_name_lens", C.POINTER(C.c_size_t))]
 
 
 class GenConfig(C.Structure):
@@ -82,7 +94,7 @@ EXPORTS = ["vlscan_device_count", "vlscan_ctx_create", "vlscan_ctx_free", "vlsca
            "vlscan_batch_upload", "vlscan_batch_free", "vlscan_batch_nblocks", "vlscan_batch_rows", "vlscan_batch_words", "vlscan_batch_device_bytes",
            "vlscan_batch_generate", "vlscan_batch_download", "vlscan_host_blocks_get", "vlscan_host_blocks_field", "vlscan_host_blocks_bytes",
            "vlscan_host_blocks_free", "vlscan_host_blocks_compress", "vlscan_zstd_decompress", "vlscan_zstd_inspect", "vlscan_zstd_walk_digest", "vlscan_part_open", "vlscan_part_free", "vlscan_part_header", "vlscan_part_nblocks", "vlscan_part_block_header", "vlscan_part_timestamps",
-           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_truncate_timestamp", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch"]
+           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_truncate_timestamp", "vlscan_last_rows", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch"]
 
 
 def lib_path():
@@ -180,6 +192,15 @@ def hits_query(step, offset=0, calendar=BUCKET_PLAIN, by=()):
     arr = (C.c_char_p * max(len(names), 1))(*names)
     lens = (C.c_size_t * max(len(names), 1))(*[len(x) for x in names])
     return HitsQuery(step, offset, calendar, len(names), arr, lens), (arr, lens)
+
+
+def last_query(limit, fields=(), min_timestamp=None):
+    """-> (vlscan_last_query, objects that must stay alive while it is used); min_timestamp None = no floor"""
+    names = [_b(f) for f in fields]
+    arr = (C.c_char_p * max(len(names), 1))(*names)
+    lens = (C.c_size_t * max(len(names), 1))(*[len(x) for x in names])
+    floor = I64_MIN if min_timestamp is None else min_timestamp
+    return LastQuery(limit, floor, len(names), arr, lens), (arr, lens)
 
 
 def parse_math_number(s):
@@ -778,6 +799,36 @@ class Ctx:
         for g in range(int(out_info[0])):
             keys = tuple(raw[int(offs[g * nby + f]):int(offs[g * nby + f + 1])] for f in range(nby))
             out.append((int(buckets[g]), keys, int(counts[g])))
+        return out
+
+    def last_rows(self, limit, fields=(), min_timestamp=None, info=None):
+        """The `limit` newest selected rows of the last scan with _time >= min_timestamp (vlscan_last_rows)
+        -> [(timestamp, block, row, (field texts as bytes...))] ascending by (timestamp, block, row).  `info` (a dict) receives rows,
+        value_bytes, selected (rows of the scan) and blocks_decoded (blocks whose timestamps had to be decoded)."""
+        q, keep = last_query(limit, fields, min_timestamp)
+        nf = len(fields)
+        cap_rows, cap_bytes = max(1, min(int(limit), 1 << 12)), 1 << 16
+        out_info = (C.c_uint64 * 4)()
+        for _ in range(2):
+            ts = np.zeros(cap_rows, dtype=np.int64)
+            blocks = np.zeros(cap_rows, dtype=np.uint32)
+            rows = np.zeros(cap_rows, dtype=np.uint32)
+            offs = np.zeros(cap_rows * nf + 1, dtype=np.uint64)
+            vb = np.zeros(max(cap_bytes, 1), dtype=np.uint8)
+            rc = lib().vlscan_last_rows(self.h, C.byref(q), ts.ctypes.data_as(C.c_void_p), blocks.ctypes.data_as(C.c_void_p), rows.ctypes.data_as(C.c_void_p),
+                                        C.c_uint64(cap_rows), vb.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes), offs.ctypes.data_as(C.c_void_p), out_info)
+            if rc and (out_info[0] > cap_rows or out_info[1] > cap_bytes):
+                cap_rows, cap_bytes = max(cap_rows, out_info[0]), max(cap_bytes, out_info[1])
+                continue
+            self._check(rc)
+            break
+        if info is not None:
+            info.update(rows=out_info[0], value_bytes=out_info[1], selected=out_info[2], blocks_decoded=out_info[3])
+        raw = vb.tobytes()
+        out = []
+        for i in range(int(out_info[0])):
+            texts = tuple(raw[int(offs[i * nf + f]):int(offs[i * nf + f + 1])] for f in range(nf))
+            out.append((int(ts[i]), int(blocks[i]), int(rows[i]), texts))
         return out
 
     def result_digest(self, block_lo, block_hi, key_base=0):
