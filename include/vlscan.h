@@ -372,6 +372,37 @@ typedef struct vlscan_last_query {
 } vlscan_last_query;
 int vlscan_last_rows(vlscan_ctx* ctx, const vlscan_last_query* q, int64_t* out_timestamps, uint32_t* out_blocks, uint32_t* out_rows, uint64_t cap_rows,
                      uint8_t* out_bytes, uint64_t cap_bytes, uint64_t* out_offsets, uint64_t out_info[4]);
+/* ---- facets: `| facets N max_values_per_field M max_value_len L` over the selected rows (/select/logsql/facets, app/vlselect/logsql/logsql.go:31-106) ----
+ * The state one pipeFacetsProcessorShard (lib/logstorage/pipe_facets.go:162-307) holds after it saw the selected rows of the last vlscan_scan_resident
+ * of the ctx; limit, the skip of const fields and the merge of batches stay with the caller (INTEGRATION.md §3e).  Same preconditions as the gather
+ * calls; the call leaves the scan result as it was.  Blocks with selected rows must have been staged with timestamps when `_time` is a field.
+ *   field_names: canonical names ("" = _msg), "_time" for the timestamps; at least one, no duplicates, no `_stream` / `_stream_id` (streams are
+ *     unknown to the engine).  A field a block does not have adds nothing for that block.
+ *   what a block adds to a field (updateFacetsForColumn): a const value with the block's selected rows as hits; each dict entry with selected rows;
+ *     every selected row's uint8..uint64 / int64 number; and the text of every other value as vlscan_gather_values yields it (`_time`: RFC3339Nano,
+ *     UTC).  Texts skip "" and are keyed like hitsMapAdaptive.updateStateGeneric: a text tryParseUint64 accepts is that number ("1_000" and a uint16
+ *     1000 are one entry), a '-' text tryParseInt64 accepts is a negative-class number ("-0" is not the uint64 0), anything else is its bytes.
+ *   dropped: a field with a value longer than max_value_len (numbers by uint64StringLen / int64StringLen when max_value_len <= 20 / 21), or with
+ *     more than max_values_per_field distinct entries.  Its state is only that flag.  A table of the next power of two >= 2 * min(max_values_per_field
+ *     + 1, selected rows) slots per field lives on the device; a max_values_per_field whose tables do not fit fails the call.
+ * Output: out_dropped[f] (0 kept, 1 dropped); the entries of field f are [out_field_offsets[f], out_field_offsets[f + 1]) (nfields + 1 offsets),
+ * ordered by hits descending, then text bytewise, then class (VLSCAN_FACET_UINT64 < _NEGATIVE < _STRING); entry e has out_hits[e], out_classes[e] and
+ * the text out_bytes[out_value_offsets[e], out_value_offsets[e + 1]) (marshalUint64String / marshalInt64String for the two number classes).
+ * out_info (may be NULL) = {entries, value bytes, selected rows, blocks whose timestamps were decoded}; it is filled also when the call fails because
+ * cap_entries or cap_bytes is too small (then nothing else is written).  `_time` decodes only blocks whose minimum differs from their maximum.
+ * At most 2^32 - 2 selected rows per batch. */
+enum { VLSCAN_FACET_UINT64 = 0, VLSCAN_FACET_NEGATIVE = 1, VLSCAN_FACET_STRING = 2 };
+#define VLSCAN_FACETS_DEFAULT_MAX_VALUES 1000    /* pipeFacetsDefaultMaxValuesPerField */
+#define VLSCAN_FACETS_DEFAULT_MAX_VALUE_LEN 128  /* pipeFacetsDefaultMaxValueLen */
+typedef struct vlscan_facets_query {
+    uint64_t max_values_per_field;   /* 0 = VLSCAN_FACETS_DEFAULT_MAX_VALUES                                                       */
+    uint64_t max_value_len;          /* 0 = VLSCAN_FACETS_DEFAULT_MAX_VALUE_LEN                                                    */
+    uint32_t nfields;
+    const char* const* field_names;
+    const size_t* field_name_lens;
+} vlscan_facets_query;
+int vlscan_facets(vlscan_ctx* ctx, const vlscan_facets_query* q, uint8_t* out_dropped, uint64_t* out_field_offsets, uint64_t* out_hits, uint8_t* out_classes,
+                  uint64_t cap_entries, uint8_t* out_bytes, uint64_t cap_bytes, uint64_t* out_value_offsets, uint64_t out_info[4]);
 /* Digest of the last scan's bitmaps of the blocks [block_lo, block_hi) of its batch, computed on the device: xor over the blocks of
  * XXH64(the block's bitmap words as little-endian bytes) * (2 * (key_base + block index) + 1).  The oracle reports the same quantity for its own
  * bitmaps, so a bench can check a billion-row scan against the CPU restatement on any block range without moving the bitmaps.  The batch of the

@@ -833,7 +833,8 @@ void vlscan_ctx_free(vlscan_ctx* ctx) {
     for (auto& r : ctx->row_off8) r.release();
     for (auto& r : ctx->ready) r.release();
     ctx->zsrc.release(); ctx->zcols.release(); ctx->ztest.release(); ctx->ts_vals.release();
-    for (DevBuf* b : {&ctx->hit_block, &ctx->glens, &ctx->goffs, &ctx->gtiles, &ctx->gout, &ctx->gstat, &ctx->hblk, &ctx->htab, &ctx->hgrp, &ctx->lcand}) b->release();
+    for (DevBuf* b : {&ctx->hit_block, &ctx->glens, &ctx->goffs, &ctx->gtiles, &ctx->gout, &ctx->gstat, &ctx->hblk, &ctx->htab, &ctx->hgrp, &ctx->lcand, &ctx->ftab}) b->release();
+    for (DevBuf& b : ctx->ftxt) b.release();
     zstd_dev_free(ctx->zdev);
     delete ctx->pool;
     if (ctx->pinned) cudaFreeHost(ctx->pinned);
@@ -1641,6 +1642,213 @@ int vlscan_last_rows(vlscan_ctx* ctx, const vlscan_last_query* q, int64_t* out_t
                 out_offsets[i * q->nfields + f + 1] = o;
             }
         }
+    });
+    if (out_info) memcpy(out_info, info, sizeof info);
+    return rc;
+}
+
+// marshalTimestampRFC3339NanoString in UTC: "2006-01-02T15:04:05" (fmt_iso8601's first 19 bytes), the fraction without its trailing zeros, "Z"
+static std::string rfc3339_nano(int64_t ts) {
+    uint8_t buf[32];
+    fmt_iso8601(buf, ts);
+    std::string s((const char*)buf, 19);
+    int64_t frac = ts % 1000000000LL;
+    if (frac < 0) frac += 1000000000LL;
+    if (frac) {
+        char f[16];
+        snprintf(f, sizeof f, ".%09lld", (long long)frac);
+        size_t n = strlen(f);
+        while (f[n - 1] == '0') n--;
+        s.append(f, n);
+    }
+    return s + "Z";
+}
+
+int vlscan_facets(vlscan_ctx* ctx, const vlscan_facets_query* q, uint8_t* out_dropped, uint64_t* out_field_offsets, uint64_t* out_hits, uint8_t* out_classes,
+                  uint64_t cap_entries, uint8_t* out_bytes, uint64_t cap_bytes, uint64_t* out_value_offsets, uint64_t out_info[4]) {
+    uint64_t info[4] = {0, 0, 0, 0};   // entries, value bytes, selected rows, blocks whose timestamps were decoded
+    const int rc = guarded(ctx, [&] {
+        if (!q) throw BadInput("no facets query");
+        if (q->nfields == 0) throw BadInput("vlscan_facets needs at least one field");
+        if (!q->field_names || !q->field_name_lens) throw BadInput("vlscan_facets: field names missing");
+        std::vector<std::string> names;
+        for (uint32_t f = 0; f < q->nfields; f++) {
+            std::string n(q->field_names[f], q->field_name_lens[f]);
+            if (n.empty()) n = "_msg";   // getCanonicalColumnName
+            if (n == "_stream" || n == "_stream_id") throw BadInput("`" + n + "` facets are not computed by the engine: it does not know the streams of the blocks");
+            if (std::find(names.begin(), names.end(), n) != names.end()) throw BadInput("duplicate facets field `" + n + "`");
+            names.push_back(n);
+        }
+        const uint64_t max_values = q->max_values_per_field ? q->max_values_per_field : VLSCAN_FACETS_DEFAULT_MAX_VALUES;
+        const uint64_t max_len = q->max_value_len ? q->max_value_len : VLSCAN_FACETS_DEFAULT_MAX_VALUE_LEN;
+        if (!ctx) throw BadInput("vlscan_facets needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
+        const uint64_t n = build_hit_list(ctx, nullptr);
+        if (n >= 0xFFFFFFFFull) throw BadInput("more than 2^32 - 2 selected rows in one batch");
+        info[2] = n;
+        const uint32_t nf = q->nfields;
+        std::vector<uint8_t> dropped(nf, 0);
+        std::vector<uint64_t> field_off(nf + 1, 0);
+        std::vector<uint64_t> ehits, evoff(1, 0);
+        std::vector<uint8_t> ecls;
+        std::string ebytes;
+        if (n) {
+            const vlscan_batch* b = ctx->last_batch;
+            BatchView B = b->view();
+            // small device state: the field table, the entry bases and cursors, a work counter, a flag, the blocks with hits
+            size_t off = 0;
+            auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 15) & ~(size_t)15; return o; };
+            const size_t o_fields = take(nf * sizeof(FacetField)), o_base = take((nf + 1) * 8), o_cursor = take(nf * 8), o_wc = take(WC_COUNT * 4), o_flag = take(4),
+                         o_blocks = take(b->nblocks * 4 + 4);
+            ctx->hblk.ensure(off);
+            uint8_t* hb = ctx->hblk.as<uint8_t>();
+            FacetField* d_fields = (FacetField*)(hb + o_fields);
+            uint64_t* d_base = (uint64_t*)(hb + o_base); unsigned long long* d_cursor = (unsigned long long*)(hb + o_cursor);
+            uint32_t* d_wc = (uint32_t*)(hb + o_wc); unsigned int* d_flag = (unsigned int*)(hb + o_flag); uint32_t* d_blocks = (uint32_t*)(hb + o_blocks);
+            VL_CUDA(cudaMemsetAsync(d_wc, 0, WC_COUNT * 4, ctx->stream));
+            k_hit_blocks_list<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), -1, 1, d_blocks, d_wc); launch_check(ctx);
+            uint32_t nblk = 0;
+            VL_CUDA(cudaMemcpyAsync(&nblk, d_wc + WC_ROW, 4, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaStreamSynchronize(ctx->stream));
+            std::vector<FacetField> hf(nf);
+            bool has_time = false;
+            if (ctx->ftxt.size() < nf) ctx->ftxt.resize(nf);
+            for (uint32_t f = 0; f < nf; f++) {
+                FacetField& F = hf[f];
+                F.is_time = names[f] == "_time";
+                F.slot = F.is_time ? -1 : field_slot(b, names[f]);
+                F.row_off8 = hit_row_offsets(ctx, F.slot);
+                F.toffs = nullptr; F.tbytes = nullptr;
+                has_time |= F.is_time;
+                if (F.slot < 0 || !nblk) continue;
+                // a field stored as float64 / ipv4 / iso8601 in a block with hits: the texts of every hit, formatted by the gather kernels first, so
+                // that no formatter runs inside the facets pass
+                unsigned int formatted = 0;
+                VL_CUDA(cudaMemsetAsync(d_flag, 0, 4, ctx->stream));
+                k_facets_formatted<<<cdiv(nblk, 256), 256, 0, ctx->stream>>>(B, d_blocks, nblk, F.slot, d_flag); launch_check(ctx);
+                VL_CUDA(cudaMemcpyAsync(&formatted, d_flag, 4, cudaMemcpyDeviceToHost, ctx->stream));
+                VL_CUDA(cudaStreamSynchronize(ctx->stream));
+                if (!formatted) continue;
+                const uint64_t total = text_offsets(ctx, F.slot, F.row_off8, ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), n);
+                text_bytes(ctx, F.slot, F.row_off8, ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), n, total);
+                DevBuf& T = ctx->ftxt[f];
+                T.ensure((n + 1) * 8 + total + 16);
+                VL_CUDA(cudaMemcpyAsync(T.p, ctx->goffs.p, (n + 1) * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+                if (total) VL_CUDA(cudaMemcpyAsync(T.as<uint8_t>() + (n + 1) * 8, ctx->gout.p, total, cudaMemcpyDeviceToDevice, ctx->stream));
+                F.toffs = T.as<uint64_t>(); F.tbytes = T.as<uint8_t>() + (n + 1) * 8;
+            }
+            // one table per field, bounded by the keys it can hold before it is dropped (saturating: max_values may be UINT64_MAX)
+            const uint64_t bound = std::min(max_values, n - 1) + 1;
+            uint64_t cap = 16;
+            while (cap < 2 * bound) cap <<= 1;
+            const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)nblk * nf, (uint64_t)ctx->sm_count * 4));
+            const uint64_t table_bytes = (uint64_t)nf * cap * 16 + nf * 16 + 64;
+            size_t free_b = 0, total_b = 0;
+            VL_CUDA(cudaMemGetInfo(&free_b, &total_b));
+            if (cap > (1ull << 40) / 16 || table_bytes > ctx->ftab.cap + free_b / 2)
+                throw BadInput("vlscan_facets: max_values_per_field = " + std::to_string(max_values) + " needs " + std::to_string(table_bytes >> 20) + " MiB of facet tables for " +
+                               std::to_string(nf) + " fields, more than the device has free");
+            ctx->ftab.ensure(table_bytes);
+            VL_CUDA(cudaMemcpyAsync(d_fields, hf.data(), nf * sizeof(FacetField), cudaMemcpyHostToDevice, ctx->stream));
+            FacetsArgs A;
+            A.fields = d_fields; A.nf = nf; A.blocks = d_blocks; A.nblocks = nblk; A.max_values = max_values; A.max_len = max_len;
+            A.hits = ctx->hits.as<uint32_t>(); A.hit_block = ctx->hit_block.as<uint32_t>(); A.hit_offs = ctx->hit_offs.as<uint64_t>(); A.counts = ctx->counts.as<uint32_t>();
+            A.tags = ctx->ftab.as<unsigned long long>(); A.cnt = A.tags + (uint64_t)nf * cap; A.nkeys = A.cnt + (uint64_t)nf * cap; A.dropped = (unsigned int*)(A.nkeys + nf);
+            A.cap = cap; A.ts_vals = nullptr;
+            VL_CUDA(cudaMemsetAsync(A.tags, 0, table_bytes, ctx->stream));
+            unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
+            uint32_t decoded = 0;
+            if (has_time) {   // timestamps of the blocks with hits that are not flat
+                uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* row_blocks = ctx->row_blocks.as<uint32_t>();
+                VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
+                k_facets_ts_list<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, A.counts, row_blocks, wc, gstat); launch_check(ctx);
+                ctx->ts_vals.ensure(b->nwords * 64 * 8);
+                k_ts_decode_list<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(B, row_blocks, wc, ctx->ts_vals.as<unsigned long long>(), gstat); launch_check(ctx);
+                VL_CUDA(cudaMemcpyAsync(&decoded, wc + WC_ROW, 4, cudaMemcpyDeviceToHost, ctx->stream));
+                A.ts_vals = ctx->ts_vals.as<unsigned long long>();
+                check_gather_errors(ctx);
+            }
+            info[3] = decoded;
+            k_facets<<<grid, 256, 0, ctx->stream>>>(B, A, gstat); launch_check(ctx);
+            std::vector<unsigned long long> nkeys(nf); std::vector<uint32_t> drop(nf);
+            VL_CUDA(cudaMemcpyAsync(nkeys.data(), A.nkeys, nf * 8, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(drop.data(), A.dropped, nf * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            check_gather_errors(ctx);   // synchronises
+            for (uint32_t f = 0; f < nf; f++) {
+                dropped[f] = drop[f] ? 1 : 0;
+                field_off[f + 1] = field_off[f] + (dropped[f] ? 0 : nkeys[f]);
+            }
+            const uint64_t E = field_off[nf];
+            std::vector<uint32_t> cls(E), rrows(E), rblocks(E); std::vector<unsigned long long> nums(E), cnts(E);
+            ctx->hgrp.ensure(E * 40 + 64);
+            uint32_t* rep_rows = ctx->hgrp.as<uint32_t>(); uint32_t* rep_blocks = rep_rows + E; uint32_t* d_cls = rep_blocks + E;
+            unsigned long long* d_nums = (unsigned long long*)(ctx->hgrp.as<uint8_t>() + ((E * 12 + 7) & ~7ull)); unsigned long long* d_cnts = d_nums + E;
+            uint32_t* str_rows = (uint32_t*)(d_cnts + E); uint32_t* str_blocks = str_rows + E;
+            if (E) {   // the entries field after field
+                VL_CUDA(cudaMemcpyAsync(d_base, field_off.data(), nf * 8, cudaMemcpyHostToDevice, ctx->stream));
+                VL_CUDA(cudaMemsetAsync(d_cursor, 0, nf * 8, ctx->stream));
+                k_facets_emit<<<grid, 256, 0, ctx->stream>>>(B, A, d_base, d_cursor, rep_rows, rep_blocks, d_cls, d_nums, d_cnts, gstat); launch_check(ctx);
+                VL_CUDA(cudaMemcpyAsync(cls.data(), d_cls, E * 4, cudaMemcpyDeviceToHost, ctx->stream));
+                VL_CUDA(cudaMemcpyAsync(nums.data(), d_nums, E * 8, cudaMemcpyDeviceToHost, ctx->stream));
+                VL_CUDA(cudaMemcpyAsync(cnts.data(), d_cnts, E * 8, cudaMemcpyDeviceToHost, ctx->stream));
+                VL_CUDA(cudaMemcpyAsync(rrows.data(), rep_rows, E * 4, cudaMemcpyDeviceToHost, ctx->stream));
+                VL_CUDA(cudaMemcpyAsync(rblocks.data(), rep_blocks, E * 4, cudaMemcpyDeviceToHost, ctx->stream));
+                check_gather_errors(ctx);
+            }
+            for (uint32_t f = 0; f < nf; f++) {
+                const uint64_t e0 = field_off[f], ne = field_off[f + 1] - e0;
+                if (!ne) continue;
+                std::vector<std::string> text(ne);
+                // the texts of the string-class representatives only
+                std::vector<uint64_t> str_of; std::vector<uint32_t> sr, sb;
+                for (uint64_t i = 0; i < ne; i++)
+                    if (cls[e0 + i] == FK_STR) { str_of.push_back(i); sr.push_back(rrows[e0 + i]); sb.push_back(rblocks[e0 + i]); }
+                std::vector<uint64_t> toffs; std::string tbytes;
+                if (!str_of.empty()) {
+                    const uint64_t ns = str_of.size();
+                    VL_CUDA(cudaMemcpyAsync(str_rows, sr.data(), ns * 4, cudaMemcpyHostToDevice, ctx->stream));
+                    VL_CUDA(cudaMemcpyAsync(str_blocks, sb.data(), ns * 4, cudaMemcpyHostToDevice, ctx->stream));
+                    const uint64_t total = text_offsets(ctx, hf[f].slot, hf[f].row_off8, str_rows, str_blocks, ns);
+                    toffs.resize(ns + 1); tbytes.resize(total);
+                    text_bytes(ctx, hf[f].slot, hf[f].row_off8, str_rows, str_blocks, ns, total);
+                    VL_CUDA(cudaMemcpyAsync(toffs.data(), ctx->goffs.p, (ns + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+                    if (total) VL_CUDA(cudaMemcpyAsync(&tbytes[0], ctx->gout.p, total, cudaMemcpyDeviceToHost, ctx->stream));
+                    check_gather_errors(ctx);
+                    for (uint64_t k = 0; k < ns; k++) text[str_of[k]] = tbytes.substr(toffs[k], toffs[k + 1] - toffs[k]);
+                }
+                std::vector<uint8_t> ecl(ne);
+                for (uint64_t i = 0; i < ne; i++) {
+                    const uint64_t e = e0 + i;
+                    char nb[24];
+                    switch (cls[e]) {
+                    case FK_U64: snprintf(nb, sizeof nb, "%llu", (unsigned long long)nums[e]); text[i] = nb; ecl[i] = VLSCAN_FACET_UINT64; break;
+                    case FK_NEG: snprintf(nb, sizeof nb, "%lld", (long long)nums[e]); text[i] = nb; ecl[i] = VLSCAN_FACET_NEGATIVE; break;
+                    case FK_TIME: text[i] = rfc3339_nano((int64_t)nums[e]); ecl[i] = VLSCAN_FACET_STRING; break;
+                    default: ecl[i] = VLSCAN_FACET_STRING;   // its text was gathered above
+                    }
+                }
+                // hits descending, then text bytewise, then class: a total order, where the reference's sort.Slice leaves ties unordered
+                std::vector<uint64_t> order(ne);
+                for (uint64_t i = 0; i < ne; i++) order[i] = i;
+                std::sort(order.begin(), order.end(), [&](uint64_t x, uint64_t y) {
+                    if (cnts[e0 + x] != cnts[e0 + y]) return cnts[e0 + x] > cnts[e0 + y];
+                    const int c = text[x].compare(text[y]);
+                    return c ? c < 0 : ecl[x] < ecl[y];
+                });
+                for (uint64_t i : order) {
+                    ehits.push_back(cnts[e0 + i]); ecls.push_back(ecl[i]);
+                    ebytes += text[i]; evoff.push_back(ebytes.size());
+                }
+            }
+        }
+        info[0] = ehits.size(); info[1] = ebytes.size();
+        if (info[0] > cap_entries) throw BadInput("facets entries buffer too small (the needed size is reported)");
+        if (info[1] > cap_bytes) throw BadInput("facets value bytes buffer too small (the needed size is reported)");
+        if (!out_dropped || !out_field_offsets || !out_value_offsets || (info[0] && (!out_hits || !out_classes)) || (info[1] && !out_bytes)) throw BadInput("facets output buffer missing");
+        memcpy(out_dropped, dropped.data(), nf);
+        memcpy(out_field_offsets, field_off.data(), (nf + 1) * 8);
+        memcpy(out_value_offsets, evoff.data(), evoff.size() * 8);
+        if (info[0]) { memcpy(out_hits, ehits.data(), info[0] * 8); memcpy(out_classes, ecls.data(), info[0]); }
+        if (info[1]) memcpy(out_bytes, ebytes.data(), info[1]);
     });
     if (out_info) memcpy(out_info, info, sizeof info);
     return rc;

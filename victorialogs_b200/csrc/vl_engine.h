@@ -95,6 +95,8 @@ struct vlscan_ctx {
     vl::DevBuf hblk, htab, hgrp;           // vlscan_hits_stats: per-block bucket + multi-bucket flag, the group table (tags, counts, state), the emitted groups;
                                            // vlscan_last_rows: per-block keys / weights / counts / offsets, the radix select states, the chosen rows
     vl::DevBuf lcand;                      // vlscan_last_rows: the candidate rows (timestamp, block, row)
+    vl::DevBuf ftab;                       // vlscan_facets: the per-field tables (tags, counts) and states
+    std::vector<vl::DevBuf> ftxt;          // vlscan_facets: per requested field, the texts of every hit when the field is stored as float64 / ipv4 / iso8601
     vl::DevBuf need;                       // bloom-first probe pass: one byte per (block, field), set when the column's values must be staged
     const void* bf_prog = nullptr; int bf_skip = 0;   // adaptive bloom-first: after a probe that pruned next to nothing, the next calls with the same program stage everything at once
     vl::DevBuf zsrc, zcols, ztest;         // compressed staging of on-disk values blocks; their column list; test output

@@ -1345,6 +1345,33 @@ static __global__ void k_gather_ts(BatchView B, const uint32_t* __restrict__ hit
     const uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (h < nhits) out[h] = (long long)ts_vals[B.blk_word_off[hit_block[h]] * 64 + hits[h]];
 }
+// The bytes of a const, strings or dict cell in row r of block b (a column of another kind: none); false for a typed column, whose text
+// must be formatted.  The decode value_text and the facets kernels share.
+static __device__ __forceinline__ bool cell_bytes(const BatchView& B, const DevColumn& c, uint32_t b, uint32_t r, const uint32_t* __restrict__ row_off8, const uint8_t** out,
+                                                  uint32_t* out_len, unsigned long long* __restrict__ stats) {
+    const uint8_t* src = nullptr; uint32_t len = 0;
+    if (c.kind == COL_CONST) { src = B.hdr + c.meta_off; len = c.meta_len; }
+    else if (c.kind == COL_VALUES) {
+        const uint8_t* data = B.arena + c.data_off;
+        if (c.vt == VT_STRING) {
+            if (c.data_const) { src = data; len = (uint32_t)c.data_len; }
+            else if (c.lens_type >= 4) { len = c.lens_const; src = data + (uint64_t)r * len; }
+            else {
+                const uint8_t* lens = B.arena + c.lens_off;
+                uint32_t o = row_off8[(B.blk_word_off[b] << 3) + (r >> 3)];
+                for (uint32_t q = r & ~7u; q < r; q++) o += row_len(c, lens, q);
+                len = row_len(c, lens, r); src = data + o;
+            }
+            if ((uint64_t)(src - data) + len > c.data_len) { len = 0; atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_LENS_MISMATCH); }
+        } else if (c.vt == VT_DICT) {
+            const uint32_t id = data[r];
+            if (id >= c.dict_len) atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_DICT_INDEX);
+            else { const uint32_t* dof = (const uint32_t*)(B.hdr + c.meta_off); src = B.hdr + c.meta_off + 4 * (c.dict_len + 1) + dof[id]; len = dof[id + 1] - dof[id]; }
+        } else return false;
+    }
+    *out = src; *out_len = len;
+    return true;
+}
 // The value of column `slot` (-1: a field the batch lacks) in row r of block b as blockResultColumn.getValues yields it: row bytes of a strings
 // column, the dictionary entry, the text form of a typed value (formatted into buf, VL_FMT_F64_MAX bytes), the const value, "" for a field the
 // block does not have.  row_off8: k_lens_offsets of the slot (strings columns with per-row lens items).  Returns the length, *out the bytes.
@@ -1353,29 +1380,11 @@ static __device__ uint32_t value_text(const BatchView& B, int slot, uint32_t b, 
     const uint8_t* src = nullptr; uint32_t len = 0;
     if (slot >= 0) {
         const DevColumn& c = B.cols[(uint64_t)b * B.nfields + slot];
-        if (c.kind == COL_CONST) { src = B.hdr + c.meta_off; len = c.meta_len; }
-        else if (c.kind == COL_VALUES) {
-            const uint8_t* data = B.arena + c.data_off;
-            if (c.vt == VT_STRING) {
-                if (c.data_const) { src = data; len = (uint32_t)c.data_len; }
-                else if (c.lens_type >= 4) { len = c.lens_const; src = data + (uint64_t)r * len; }
-                else {
-                    const uint8_t* lens = B.arena + c.lens_off;
-                    uint32_t o = row_off8[(B.blk_word_off[b] << 3) + (r >> 3)];
-                    for (uint32_t q = r & ~7u; q < r; q++) o += row_len(c, lens, q);
-                    len = row_len(c, lens, r); src = data + o;
-                }
-                if ((uint64_t)(src - data) + len > c.data_len) { len = 0; atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_LENS_MISMATCH); }
-            } else if (c.vt == VT_DICT) {
-                const uint32_t id = data[r];
-                if (id >= c.dict_len) atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_DICT_INDEX);
-                else { const uint32_t* dof = (const uint32_t*)(B.hdr + c.meta_off); src = B.hdr + c.meta_off + 4 * (c.dict_len + 1) + dof[id]; len = dof[id + 1] - dof[id]; }
-            } else {
-                const uint32_t w = width_of_vt(c.vt);
-                const uint64_t raw = load_fixed_be(data + (uint64_t)r * w, w);
-                const int n = c.vt == VT_FLOAT64 ? fmt_f64(buf, raw) : encoded_to_string(c.vt, raw, buf);
-                src = buf; len = n > 0 ? (uint32_t)n : 0;
-            }
+        if (!cell_bytes(B, c, b, r, row_off8, &src, &len, stats)) {
+            const uint32_t w = width_of_vt(c.vt);
+            const uint64_t raw = load_fixed_be(B.arena + c.data_off + (uint64_t)r * w, w);
+            const int n = c.vt == VT_FLOAT64 ? fmt_f64(buf, raw) : encoded_to_string(c.vt, raw, buf);
+            src = buf; len = n > 0 ? (uint32_t)n : 0;
         }
     }
     *out = src;
@@ -1887,6 +1896,279 @@ static __global__ void k_last_choose(const long long* __restrict__ cts, const ui
     const unsigned long long p = atomicAdd(out_n, 1ull);
     out_ts[p] = t; out_blk[p] = cblk[i]; out_row[p] = crow[i];
     blk_mark[cblk[i]] = 1;
+}
+
+// ---- `| facets` over the selected rows: the state of one pipeFacetsProcessorShard that saw them (lib/logstorage/pipe_facets.go:162-282) -----------
+// A key is (class, 64-bit number) for FK_U64 / FK_NEG (the u64 and negative64 maps of hitsMapAdaptive, hits_map.go:85-115) and FK_TIME (`_time`:
+// its RFC3339Nano text is a function of the timestamp), or its text for FK_STR.  Every field has an open-addressing table of `cap` slots whose slot
+// holds only a 64-bit tag: the high half of the key's hash and 1 + the hit index of a representative row.  A probe whose hash half matches derives
+// the representative's key again and compares it (texts byte for byte), so a hash collision costs a probe, never a wrong count.  Claiming key
+// number max_values + 1 drops the field; cap >= 2 * min(max_values + 1, selected rows), so a table never fills.
+enum { FK_U64 = 0, FK_NEG = 1, FK_STR = 2, FK_TIME = 3 };
+enum { FR_SKIP = 0, FR_OK = 1, FR_DROP = 2 };
+#define VL_FACET_SLOTS 1024   // per-CTA pre-aggregation table of a (field, block) work item; it takes new keys up to half full
+struct FacetField {
+    int slot, is_time;                       // slot -1: no block of the batch has the field
+    const uint32_t* row_off8;                // k_lens_offsets of the slot
+    const uint64_t* toffs; const uint8_t* tbytes;   // texts of every hit (k_gather_values) when a block with hits stores the field as float64 / ipv4 / iso8601
+};
+struct FacetsArgs {
+    const FacetField* fields; uint32_t nf;
+    const uint32_t* blocks; uint32_t nblocks;   // the blocks with hits
+    uint64_t max_values, max_len;
+    const uint32_t* hits; const uint32_t* hit_block; const uint64_t* hit_offs; const uint32_t* counts;   // build_hit_list
+    const unsigned long long* ts_vals;       // k_ts_decode_list of the blocks with hits whose timestamps are not all equal
+    unsigned long long* tags; unsigned long long* cnt;   // [nf * cap]
+    unsigned long long* nkeys; unsigned int* dropped;    // [nf]
+    uint64_t cap;
+};
+struct FKey { uint32_t cls, len; uint64_t num, hash; const uint8_t* src; };
+
+// uint64StringLen / int64StringLen (pipe_facets.go:240-282): 20 for every n >= 10^10
+static __device__ __forceinline__ uint32_t facet_u64_len(uint64_t n) {
+    if (n >= 10000000000ull) return 20;
+    uint32_t k = 1;
+    for (uint64_t p = 10; n >= p; p *= 10) k++;
+    return k;
+}
+static __device__ __forceinline__ uint32_t facet_i64_len(int64_t v) {
+    if (v >= 0) return facet_u64_len((uint64_t)v);
+    return v == INT64_MIN ? 21 : 1 + facet_u64_len((uint64_t)(-v));
+}
+// length of marshalTimestampRFC3339NanoString in UTC: "2006-01-02T15:04:05Z", plus "." and the fraction without its trailing zeros
+static __device__ __forceinline__ uint32_t facet_rfc3339_len(int64_t ts) {
+    int64_t frac = ts % 1000000000LL;
+    if (frac < 0) frac += 1000000000LL;
+    if (!frac) return 20;
+    uint32_t len = 30;
+    while (frac % 10 == 0) { frac /= 10; len--; }
+    return len;
+}
+static __device__ __forceinline__ void facet_num_key(FKey& k, uint32_t cls, uint64_t num) {
+    k.cls = cls; k.num = num; k.src = nullptr; k.len = 0; k.hash = mix64(num ^ (0x9E3779B97F4A7C15ull * (cls + 1)));
+}
+// hitsMapAdaptive.updateStateGeneric (hits_map.go:85-97): tryParseUint64, then a '-' text through tryParseInt64, else the bytes
+static __device__ __forceinline__ void facet_text_key(FKey& k, const uint8_t* s, uint32_t n) {
+    uint64_t v;
+    if (mn::parse_u64(mn::Span{s, n}, &v)) { facet_num_key(k, FK_U64, v); return; }
+    if (n > 1 && s[0] == '-' && mn::parse_u64(mn::Span{s + 1, n - 1}, &v) && v <= (1ull << 63)) { facet_num_key(k, FK_NEG, 0ull - v); return; }
+    uint64_t h = 0xCBF29CE484222325ull;
+    for (uint32_t i = 0; i < n; i++) h = (h ^ s[i]) * 0x100000001B3ull;
+    k.cls = FK_STR; k.num = 0; k.src = s; k.len = n; k.hash = mix64(h ^ n);
+}
+// the key of field F in hit h = row r of block b.  FR_SKIP: no key (an empty value, a field the block does not have); FR_DROP: the value is
+// too long for max_value_len, which drops the field (updateStateGeneric / updateStateUint64 / updateStateInt64, pipe_facets.go:222-307).
+// float64 / ipv4 / iso8601 texts come from F.tbytes, formatted before the pass: no formatter runs here.
+static __device__ __forceinline__ int facet_row_key(const BatchView& B, const FacetsArgs& A, const FacetField& F, uint32_t b, uint32_t r, uint64_t h, FKey& k,
+                                                    unsigned long long* __restrict__ stats) {
+    if (F.is_time) {
+        const DevTimestamps& t = B.ts[b];
+        const int64_t ts = t.first == t.max ? t.first : (int64_t)A.ts_vals[B.blk_word_off[b] * 64 + r];
+        facet_num_key(k, FK_TIME, (uint64_t)ts);
+        return facet_rfc3339_len(ts) > A.max_len ? FR_DROP : FR_OK;
+    }
+    if (F.slot < 0) return FR_SKIP;
+    const DevColumn& c = B.cols[(uint64_t)b * B.nfields + F.slot];
+    const uint8_t* src; uint32_t len;
+    if (!cell_bytes(B, c, b, r, F.row_off8, &src, &len, stats)) {
+        if (c.vt == VT_UINT8 || c.vt == VT_UINT16 || c.vt == VT_UINT32 || c.vt == VT_UINT64 || c.vt == VT_INT64) {
+            const uint32_t w = width_of_vt(c.vt);
+            const uint64_t raw = load_fixed_be(B.arena + c.data_off + (uint64_t)r * w, w);
+            if (c.vt != VT_INT64) {
+                facet_num_key(k, FK_U64, raw);
+                return A.max_len <= 20 && facet_u64_len(raw) > A.max_len ? FR_DROP : FR_OK;
+            }
+            const int64_t v = unzigzag64(raw);
+            facet_num_key(k, v >= 0 ? FK_U64 : FK_NEG, (uint64_t)v);
+            return A.max_len <= 21 && facet_i64_len(v) > A.max_len ? FR_DROP : FR_OK;
+        }
+        if (!F.toffs) return FR_SKIP;
+        src = F.tbytes + F.toffs[h]; len = (uint32_t)(F.toffs[h + 1] - F.toffs[h]);
+    }
+    if (len == 0) return FR_SKIP;
+    if (len > A.max_len) return FR_DROP;
+    facet_text_key(k, src, len);
+    return FR_OK;
+}
+static __device__ __forceinline__ bool facet_same_key(const BatchView& B, const FacetsArgs& A, const FacetField& F, const FKey& k, uint64_t h,
+                                                      unsigned long long* __restrict__ stats) {
+    FKey o;
+    if (facet_row_key(B, A, F, A.hit_block[h], A.hits[h], h, o, stats) != FR_OK || o.cls != k.cls) return false;
+    if (k.cls != FK_STR) return o.num == k.num;
+    if (o.len != k.len) return false;
+    for (uint32_t i = 0; i < k.len; i++) if (o.src[i] != k.src[i]) return false;
+    return true;
+}
+// count c rows of key k (representative: hit `rep` = row r of block b) in the table tags / cnt of mask + 1 slots.  The per-field table (dropped !=
+// NULL) drops the field when it claims key number `limit` + 1 or finds no slot; a CTA's table (dropped == NULL) declines a new key once `limit` keys
+// are in it and returns false.
+static __device__ __forceinline__ bool facet_add(const BatchView& B, const FacetsArgs& A, const FacetField& F, unsigned long long* tags, unsigned long long* cnt, uint64_t mask,
+                                 unsigned long long* nkeys, uint64_t limit, unsigned int* dropped, const FKey& k, uint64_t rep, uint64_t c,
+                                 unsigned long long* __restrict__ stats) {
+    const unsigned long long tag = (k.hash & 0xFFFFFFFF00000000ull) | (rep + 1);
+    uint64_t s = k.hash & mask;
+    for (uint64_t p = 0; p <= mask; p++, s = (s + 1) & mask) {
+        unsigned long long cur = *(volatile unsigned long long*)&tags[s];
+        if (cur == 0) {
+            if (!dropped && *(volatile unsigned long long*)nkeys >= limit) return false;
+            cur = atomicCAS(&tags[s], 0ull, tag);
+            if (cur == 0) {
+                if (atomicAdd(nkeys, 1ull) >= limit && dropped) atomicExch(dropped, 1u);
+                atomicAdd(&cnt[s], (unsigned long long)c);
+                return true;
+            }
+        }
+        if ((cur >> 32) != (k.hash >> 32)) continue;
+        const uint64_t rh = (cur & 0xFFFFFFFFull) - 1;
+        if (facet_same_key(B, A, F, k, rh, stats)) { atomicAdd(&cnt[s], (unsigned long long)c); return true; }
+    }
+    if (!dropped) return false;
+    atomicExch(dropped, 1u);
+    return true;
+}
+static __device__ __forceinline__ void facet_add_global(const BatchView& B, const FacetsArgs& A, const FacetField& F, uint32_t f, const FKey& k, uint64_t rep, uint64_t c,
+                                                        unsigned long long* __restrict__ stats) {
+    if (*(volatile unsigned int*)&A.dropped[f]) return;
+    facet_add(B, A, F, A.tags + (uint64_t)f * A.cap, A.cnt + (uint64_t)f * A.cap, A.cap - 1, &A.nkeys[f], A.max_values, &A.dropped[f], k, rep, c, stats);
+}
+
+// Blocks with hits whose timestamps are not all equal (minimum != maximum): the decode list of the `_time` facet.  Flat blocks are one key each.
+static __global__ void k_facets_ts_list(BatchView B, const uint32_t* __restrict__ counts, uint32_t* __restrict__ row_blocks, uint32_t* __restrict__ work_count,
+                                        unsigned long long* __restrict__ stats) {
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B.nblocks || counts[b] == 0) return;
+    if (!B.ts || B.ts[b].mt == 0) { atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_NO_TIMESTAMPS); return; }
+    if (B.ts[b].first != B.ts[b].max) row_blocks[atomicAdd(&work_count[WC_ROW], 1u)] = b;
+}
+
+// 1 in *flag when a block with hits stores column `slot` as float64 / ipv4 / iso8601: the field's texts are then formatted before the pass
+static __global__ void k_facets_formatted(BatchView B, const uint32_t* __restrict__ blocks, uint32_t nblocks, int slot, unsigned int* __restrict__ flag) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nblocks) return;
+    const DevColumn& c = B.cols[(uint64_t)blocks[i] * B.nfields + slot];
+    if (c.kind == COL_VALUES && (c.vt == VT_FLOAT64 || c.vt == VT_IPV4 || c.vt == VT_ISO8601)) *flag = 1;
+}
+
+// One CTA per (block with hits, field) work item, after a look at the field's dropped flag.  A const cell and a flat `_time` cell are one insert of
+// the block's count; a dict cell counts its ids in shared memory and inserts each entry with hits once (forEachDictValueWithHits,
+// block_result.go:2381-2400); `_time` rows merge runs of equal timestamps inside each warp; other cells count their rows in a CTA table first and
+// insert each of its keys once.  Row loops look at the dropped flag again every blockDim.x rows.
+static __global__ void __launch_bounds__(256) k_facets(BatchView B, FacetsArgs A, unsigned long long* __restrict__ stats) {
+    __shared__ unsigned long long s_tag[VL_FACET_SLOTS], s_cnt[VL_FACET_SLOTS];
+    __shared__ unsigned long long s_used;
+    __shared__ uint32_t s_dcnt[8], s_drep[8];
+    __shared__ uint32_t s_stop;
+    const uint64_t nitems = (uint64_t)A.nblocks * A.nf;
+    for (uint64_t j = blockIdx.x; j < nitems; j += gridDim.x) {
+        const uint32_t b = A.blocks[j / A.nf], f = (uint32_t)(j % A.nf);
+        const uint32_t n = A.counts[b];
+        const FacetField F = A.fields[f];
+        if (F.is_time ? (!B.ts || B.ts[b].mt == 0) : F.slot < 0) continue;
+        __syncthreads();   // the previous item is done with the shared state
+        if (threadIdx.x == 0) { s_stop = *(volatile unsigned int*)&A.dropped[f]; s_used = 0; }
+        __syncthreads();
+        if (s_stop) continue;
+        const uint64_t h0 = A.hit_offs[b];
+        const DevColumn* c = F.is_time ? nullptr : &B.cols[(uint64_t)b * B.nfields + F.slot];
+        if (c && c->kind != COL_CONST && c->kind != COL_VALUES) continue;
+        FKey k;
+        if (F.is_time ? B.ts[b].first == B.ts[b].max : c->kind == COL_CONST) {   // one key for the whole block
+            if (threadIdx.x == 0) {
+                const int fr = facet_row_key(B, A, F, b, A.hits[h0], h0, k, stats);
+                if (fr == FR_DROP) atomicExch(&A.dropped[f], 1u);
+                else if (fr == FR_OK) facet_add_global(B, A, F, f, k, h0, n, stats);
+            }
+            continue;
+        }
+        if (!F.is_time && c->vt == VT_DICT) {
+            if (threadIdx.x < 8) { s_dcnt[threadIdx.x] = 0; s_drep[threadIdx.x] = 0xFFFFFFFFu; }
+            __syncthreads();
+            const uint8_t* ids = B.arena + c->data_off;
+            for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+                const uint32_t id = ids[A.hits[h0 + i]];
+                if (id >= c->dict_len || id >= 8) { atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_DICT_INDEX); continue; }
+                atomicAdd(&s_dcnt[id], 1u); atomicMin(&s_drep[id], i);
+            }
+            __syncthreads();
+            if (threadIdx.x < c->dict_len && s_dcnt[threadIdx.x]) {
+                const uint64_t rep = h0 + s_drep[threadIdx.x];
+                const int fr = facet_row_key(B, A, F, b, A.hits[rep], rep, k, stats);
+                if (fr == FR_DROP) atomicExch(&A.dropped[f], 1u);
+                else if (fr == FR_OK) facet_add_global(B, A, F, f, k, rep, s_dcnt[threadIdx.x], stats);
+            }
+            continue;
+        }
+        if (F.is_time) {   // non-decreasing in practice: runs of equal timestamps become one insert
+            const uint32_t lane = lane_id();
+            for (uint32_t base = 0; base < n; base += blockDim.x) {
+                if (base) {
+                    __syncthreads();
+                    if (threadIdx.x == 0 && *(volatile unsigned int*)&A.dropped[f]) s_stop = 1;
+                    __syncthreads();
+                    if (s_stop) break;
+                }
+                const uint32_t i = base + threadIdx.x;
+                const bool valid = i < n;
+                int fr = FR_SKIP;
+                if (valid) fr = facet_row_key(B, A, F, b, A.hits[h0 + i], h0 + i, k, stats);
+                if (fr == FR_DROP) atomicExch(&A.dropped[f], 1u);
+                const int ok = fr == FR_OK;
+                const uint64_t key = ok ? k.num : 0;
+                const uint64_t pk = __shfl_up_sync(0xffffffffu, key, 1);
+                const int pok = __shfl_up_sync(0xffffffffu, ok, 1);
+                const int same_prev = lane > 0 && ok && pok && pk == key;
+                const uint32_t heads = __ballot_sync(0xffffffffu, ok && !same_prev);
+                int same_next = __shfl_down_sync(0xffffffffu, same_prev, 1);
+                if (lane == 31) same_next = 0;
+                if (ok && !same_next) {
+                    const uint32_t head = 31 - __clz(heads & (0xffffffffu >> (31 - lane)));
+                    facet_add_global(B, A, F, f, k, h0 + i - (lane - head), lane - head + 1, stats);
+                }
+            }
+            continue;
+        }
+        for (uint32_t s = threadIdx.x; s < VL_FACET_SLOTS; s += blockDim.x) { s_tag[s] = 0; s_cnt[s] = 0; }
+        __syncthreads();
+        for (uint32_t base = 0; base < n; base += blockDim.x) {
+            if (base) {
+                __syncthreads();
+                if (threadIdx.x == 0 && *(volatile unsigned int*)&A.dropped[f]) s_stop = 1;
+                __syncthreads();
+                if (s_stop) break;
+            }
+            const uint32_t i = base + threadIdx.x;
+            if (i >= n) continue;
+            const int fr = facet_row_key(B, A, F, b, A.hits[h0 + i], h0 + i, k, stats);
+            if (fr == FR_DROP) { atomicExch(&A.dropped[f], 1u); s_stop = 1; }
+            else if (fr == FR_OK && !facet_add(B, A, F, s_tag, s_cnt, VL_FACET_SLOTS - 1, &s_used, VL_FACET_SLOTS / 2, nullptr, k, h0 + i, 1, stats))
+                facet_add_global(B, A, F, f, k, h0 + i, 1, stats);
+        }
+        __syncthreads();
+        if (s_stop) continue;
+        for (uint32_t s = threadIdx.x; s < VL_FACET_SLOTS; s += blockDim.x) {
+            const unsigned long long tag = s_tag[s];
+            if (!tag) continue;
+            const uint64_t rep = (tag & 0xFFFFFFFFull) - 1;
+            if (facet_row_key(B, A, F, b, A.hits[rep], rep, k, stats) == FR_OK) facet_add_global(B, A, F, f, k, rep, s_cnt[s], stats);
+        }
+    }
+}
+// occupied slots of the fields that were not dropped -> entries, field after field from base[f]: representative (row, block), class, number, hits
+static __global__ void __launch_bounds__(256) k_facets_emit(BatchView B, FacetsArgs A, const uint64_t* __restrict__ base, unsigned long long* __restrict__ cursor,
+                                                            uint32_t* __restrict__ rep_rows, uint32_t* __restrict__ rep_blocks, uint32_t* __restrict__ cls,
+                                                            unsigned long long* __restrict__ nums, unsigned long long* __restrict__ hits_out, unsigned long long* __restrict__ stats) {
+    const uint64_t total = (uint64_t)A.nf * A.cap;
+    for (uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; s < total; s += (uint64_t)gridDim.x * blockDim.x) {
+        const unsigned long long tag = A.tags[s];
+        const uint32_t f = (uint32_t)(s / A.cap);
+        if (!tag || A.dropped[f]) continue;
+        const uint64_t rep = (tag & 0xFFFFFFFFull) - 1;
+        const uint32_t b = A.hit_block[rep], r = A.hits[rep];
+        FKey k;
+        facet_row_key(B, A, A.fields[f], b, r, rep, k, stats);
+        const uint64_t e = base[f] + atomicAdd(&cursor[f], 1ull);
+        rep_rows[e] = r; rep_blocks[e] = b; cls[e] = k.cls; nums[e] = k.num; hits_out[e] = A.cnt[s];
+    }
 }
 
 }  // namespace vl

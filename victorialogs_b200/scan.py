@@ -84,6 +84,15 @@ class LastQuery(C.Structure):
                 ("field_names", C.POINTER(C.c_char_p)), ("field_name_lens", C.POINTER(C.c_size_t))]
 
 
+class FacetsQuery(C.Structure):
+    _fields_ = [("max_values_per_field", C.c_uint64), ("max_value_len", C.c_uint64), ("nfields", C.c_uint32),
+                ("field_names", C.POINTER(C.c_char_p)), ("field_name_lens", C.POINTER(C.c_size_t))]
+
+
+FACET_UINT64, FACET_NEGATIVE, FACET_STRING = 0, 1, 2
+FACETS_DEFAULT_MAX_VALUES, FACETS_DEFAULT_MAX_VALUE_LEN = 1000, 128
+
+
 class GenConfig(C.Structure):
     _fields_ = [("seed", C.c_uint64), ("total_rows", C.c_uint64), ("rows_per_block", C.c_uint32), ("hot_block_permille", C.c_uint32),
                 ("hit_row_permille", C.c_uint32), ("columns_mask", C.c_uint32)]
@@ -94,7 +103,7 @@ EXPORTS = ["vlscan_device_count", "vlscan_ctx_create", "vlscan_ctx_free", "vlsca
            "vlscan_batch_upload", "vlscan_batch_free", "vlscan_batch_nblocks", "vlscan_batch_rows", "vlscan_batch_words", "vlscan_batch_device_bytes",
            "vlscan_batch_generate", "vlscan_batch_download", "vlscan_host_blocks_get", "vlscan_host_blocks_field", "vlscan_host_blocks_bytes",
            "vlscan_host_blocks_free", "vlscan_host_blocks_compress", "vlscan_zstd_decompress", "vlscan_zstd_inspect", "vlscan_zstd_walk_digest", "vlscan_part_open", "vlscan_part_free", "vlscan_part_header", "vlscan_part_nblocks", "vlscan_part_block_header", "vlscan_part_timestamps",
-           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_truncate_timestamp", "vlscan_last_rows", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch"]
+           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_truncate_timestamp", "vlscan_last_rows", "vlscan_facets", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch"]
 
 
 def lib_path():
@@ -201,6 +210,44 @@ def last_query(limit, fields=(), min_timestamp=None):
     lens = (C.c_size_t * max(len(names), 1))(*[len(x) for x in names])
     floor = I64_MIN if min_timestamp is None else min_timestamp
     return LastQuery(limit, floor, len(names), arr, lens), (arr, lens)
+
+
+def facets_query(fields, max_values_per_field=0, max_value_len=0):
+    """-> (vlscan_facets_query, objects that must stay alive while it is used); 0 = the endpoint's default (1000 values, 128 bytes)"""
+    names = [_b(f) for f in fields]
+    arr = (C.c_char_p * max(len(names), 1))(*names)
+    lens = (C.c_size_t * max(len(names), 1))(*[len(x) for x in names])
+    return FacetsQuery(max_values_per_field, max_value_len, len(names), arr, lens), (arr, lens)
+
+
+def facets_merge(states, limit=10, keep_const_fields=False, max_values_per_field=0):
+    """The merge a caller runs over the per-batch states of Ctx.facets (pipeFacetsProcessor.flush, lib/logstorage/pipe_facets.go:338-420, with
+    concurrency 1) -> [(field name, value text, hits)] ordered by field name bytewise, then by hits descending.
+
+    states: [(state, selected rows)], state = {field: None (dropped) or [(class, text, hits)]} as Ctx.facets returns it, called with
+    max_values_per_field (0 = default).  A field is dropped when a batch dropped it or when its merged entries outnumber max_values_per_field; a field whose single entry covers every selected row is skipped unless keep_const_fields; ties of hits go by text, then
+    class (FACET_UINT64 < FACET_NEGATIVE < FACET_STRING)."""
+    rows = sum(n for _, n in states)
+    max_values = max_values_per_field or FACETS_DEFAULT_MAX_VALUES
+    merged, dropped = {}, set()
+    for st, _ in states:
+        for field, entries in st.items():
+            if entries is None:
+                dropped.add(field)
+                continue
+            m = merged.setdefault(field, {})
+            for cls, text, hits in entries:
+                m[(cls, text)] = m.get((cls, text), 0) + hits
+    out = []
+    for field in sorted(merged.keys() - dropped):
+        m = merged[field]
+        if len(m) > max_values:
+            continue
+        if len(m) == 1 and next(iter(m.values())) == rows and not keep_const_fields:
+            continue
+        ents = sorted(m.items(), key=lambda kv: (-kv[1], kv[0][1], kv[0][0]))[:limit]
+        out.extend((field, text, hits) for (cls, text), hits in ents)
+    return out
 
 
 def parse_math_number(s):
@@ -830,6 +877,37 @@ class Ctx:
             texts = tuple(raw[int(offs[i * nf + f]):int(offs[i * nf + f + 1])] for f in range(nf))
             out.append((int(ts[i]), int(blocks[i]), int(rows[i]), texts))
         return out
+
+    def facets(self, fields, max_values_per_field=0, max_value_len=0, info=None):
+        """The facets state of the selected rows of the last scan (vlscan_facets) -> {field: None when dropped, else [(class, text as bytes,
+        hits)] by hits descending, then text, then class}; field keys are the names as given.
+        `info` (a dict) receives entries, value_bytes, rows (selected) and blocks_decoded (blocks whose timestamps had to be decoded)."""
+        q, keep = facets_query(fields, max_values_per_field, max_value_len)
+        nf = len(fields)
+        cap_entries, cap_bytes = 1 << 12, 1 << 16
+        out_info = (C.c_uint64 * 4)()
+        for _ in range(2):
+            dropped = np.zeros(max(nf, 1), dtype=np.uint8)
+            foffs = np.zeros(nf + 1, dtype=np.uint64)
+            hits = np.zeros(cap_entries, dtype=np.uint64)
+            cls = np.zeros(cap_entries, dtype=np.uint8)
+            voffs = np.zeros(cap_entries + 1, dtype=np.uint64)
+            vb = np.zeros(max(cap_bytes, 1), dtype=np.uint8)
+            rc = lib().vlscan_facets(self.h, C.byref(q), dropped.ctypes.data_as(C.c_void_p), foffs.ctypes.data_as(C.c_void_p), hits.ctypes.data_as(C.c_void_p),
+                                     cls.ctypes.data_as(C.c_void_p), C.c_uint64(cap_entries), vb.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes),
+                                     voffs.ctypes.data_as(C.c_void_p), out_info)
+            if rc and (out_info[0] > cap_entries or out_info[1] > cap_bytes):
+                cap_entries, cap_bytes = max(cap_entries, out_info[0]), max(cap_bytes, out_info[1])
+                continue
+            self._check(rc)
+            break
+        if info is not None:
+            info.update(entries=out_info[0], value_bytes=out_info[1], rows=out_info[2], blocks_decoded=out_info[3])
+        raw = vb.tobytes()
+        state = {}
+        for f, name in enumerate(fields):
+            state[name] = None if dropped[f] else [(int(cls[e]), raw[int(voffs[e]):int(voffs[e + 1])], int(hits[e])) for e in range(int(foffs[f]), int(foffs[f + 1]))]
+        return state
 
     def result_digest(self, block_lo, block_hi, key_base=0):
         """xor over blocks of XXH64(bitmap words) * (2 * (key_base + block) + 1) of the last scan, computed on the device (vlscan_result_digest)"""
