@@ -433,6 +433,32 @@ int vlscan_result_device_ptrs(vlscan_ctx* ctx, void** bitmap_words, void** match
 int vlscan_scan_batch(vlscan_ctx* ctx, const vlscan_program* prog, const char* const* field_names, const size_t* field_name_lens,
                       uint32_t nfields, const vlscan_block* blocks, uint64_t nblocks, uint64_t* out_bitmap_words,
                       uint32_t* out_match_counts, vlscan_stats* stats);
+/* ---- keeping an end-to-end scan on the device: the pipes' columns staged only for the blocks that need them (DESIGN.md §3.12) -----------------
+ * The reference reads the columns the pipes need only after the filter left a non-empty bitmap (block_search.go:217-225).
+ * vlscan_scan_batch_keep: vlscan_scan_batch with the same arguments, bitmaps, counts and counters, whose batch stays the ctx's last result: the
+ *   gather calls, vlscan_fetch_*, vlscan_result_digest, vlscan_hits_stats, vlscan_last_rows and vlscan_facets work on it until the next
+ *   vlscan_scan_resident, vlscan_scan_batch or vlscan_scan_batch_keep on the ctx, or vlscan_ctx_free.  The device memory is the ctx's and is reused
+ *   by the next call.  The field list may name fields the program does not reference (output fields).  Staging is always split into headers and
+ *   values: const values and dict tables of every field go with the headers; the values of the program's fields are staged for the blocks the
+ *   bloom probe lets through (when the program probes and VLSCAN_BLOOM_FIRST lets it, as in vlscan_scan_batch) or for every block; the values of
+ *   output fields stay on the host.  Timestamps are staged for every block that has them.  The counters are vlscan_scan_batch's except for
+ *   h2d_bytes, gpu_launches and the timings: staged_columns / pruned_columns are filled when the bloom probe ran, 0 / 0 otherwise.  An empty
+ *   field list or an empty batch is accepted as by vlscan_scan_batch.
+ * vlscan_stage_selected: stages the values of the named fields of the kept batch for the listed blocks (block_list, nlist entries) or, with
+ *   block_list == NULL, for every block with selected rows.  `blocks` / `nblocks` must be the descriptors the keep call was given (the library
+ *   never retains caller pointers): block count, and for the blocks read, rows, column count, and per column field, kind, value type, stage
+ *   and payload lengths (on-disk: the values bytes; decoded: lens items and data, each) are checked against what that call saw (<0 on a mismatch).  Cells already staged, const cells and absent fields are
+ *   skipped; a field the kept batch was not staged with is an error, and so is an empty field list (a caller with nothing to stage skips the
+ *   call).  May be called several times; what it stages lives as long as the kept
+ *   batch.  out_info (filled on success) = {cells staged, cells skipped because already staged, host->device bytes, bytes blocks (ZSTD or
+ *   plain) run through the device decoder}.
+ * A gather, vlscan_hits_stats, vlscan_last_rows or vlscan_facets that needs the values of a cell still on the host fails with an error naming
+ * the field; the ctx and the kept result stay usable.  A failure of vlscan_stage_selected while it stages ends the kept result. */
+int vlscan_scan_batch_keep(vlscan_ctx* ctx, const vlscan_program* prog, const char* const* field_names, const size_t* field_name_lens,
+                           uint32_t nfields, const vlscan_block* blocks, uint64_t nblocks, uint64_t* out_bitmap_words,
+                           uint32_t* out_match_counts, vlscan_stats* stats);
+int vlscan_stage_selected(vlscan_ctx* ctx, const vlscan_block* blocks, uint64_t nblocks, const char* const* field_names, const size_t* field_name_lens,
+                          uint32_t nfields, const uint32_t* block_list /* NULL = every block with selected rows */, uint64_t nlist, uint64_t out_info[4]);
 
 #ifdef __cplusplus
 }

@@ -166,24 +166,30 @@ static int host_threads() {
 // UP_HEADERS stages what the header dispatch and the bloom probes look at (const values, bloom filters, dict tables -> batch->harena) and
 // leaves every values payload on the host (VALUES_DEFERRED); UP_VALUES then stages the timestamps and the values of the columns the probe marked in
 // `need` (-> batch->arena) and flags the others VALUES_ABSENT.
-enum UploadMode { UP_FULL = 0, UP_HEADERS = 1, UP_VALUES = 2 };
+// UP_LATE (vlscan_stage_selected on a kept batch) stages the values of the columns marked in `need` into a new region of the batch
+// (batch->late), leaves every other cell as it is and rewrites only the staged cells' entries of the device column table.
+enum UploadMode { UP_FULL = 0, UP_HEADERS = 1, UP_VALUES = 2, UP_LATE = 3 };
 static void do_upload(vlscan_ctx* ctx, const char* const* field_names, const size_t* field_name_lens, uint32_t nfields, const vlscan_block* blocks,
                       uint64_t nblocks, vlscan_batch* out, vlscan_stats* stats, const std::vector<char>* need_bloom = nullptr, UploadMode mode = UP_FULL,
-                      const uint8_t* need = nullptr) {
+                      const uint8_t* need = nullptr, uint64_t* zframes = nullptr) {
     VL_CUDA(cudaSetDevice(ctx->device));
     if (nblocks > 0xFFFFFFF0ull) throw BadInput("too many blocks in one batch");
     const bool dbg = getenv("VLSCAN_DEBUG_TIMING") != nullptr;
     auto now = [] { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
     double t_start = now(), t_desc = 0, t_alloc = 0, t_copy = 0;
     out->device = ctx->device; out->nfields = nfields;
-    std::vector<DevColumn>& cols = out->h_cols;   // UP_VALUES continues with the table UP_HEADERS left
-    if (mode != UP_VALUES) {
+    std::vector<DevColumn>& cols = out->h_cols;   // UP_VALUES and UP_LATE continue with the table UP_HEADERS left
+    const bool values_phase = mode == UP_VALUES || mode == UP_LATE;
+    if (!values_phase) {
         for (uint32_t f = 0; f < nfields; f++) out->field_names.emplace_back(field_names[f], field_name_lens[f]);
         cols.assign((size_t)nblocks * std::max<uint32_t>(nfields, 1), DevColumn{});
         memset(cols.data(), 0, cols.size() * sizeof(DevColumn));
+        out->late_used = 0;   // a new batch: the late regions of the previous one are free
     } else if (cols.size() != (size_t)nblocks * std::max<uint32_t>(nfields, 1) || !need) throw BadInput("internal: values phase of a bloom-first upload without its header phase");
     out->split_hdr = mode != UP_FULL;
-    DevBuf& arena_buf = mode == UP_HEADERS ? out->harena : out->arena;
+    if (mode == UP_LATE && out->late_used == out->late.size()) out->late.emplace_back();
+    DevBuf& arena_buf = mode == UP_HEADERS ? out->harena : mode == UP_LATE ? out->late[out->late_used] : out->arena;
+    std::vector<uint64_t> late_cells;   // UP_LATE: the cells staged by this call
     std::vector<uint32_t> rows(nblocks);
     struct Piece { const uint8_t* src; uint64_t len; uint64_t dst; };
     std::vector<Piece> pieces, zpieces;   // host -> arena, host -> compressed staging (on-disk values blocks)
@@ -343,10 +349,10 @@ static void do_upload(vlscan_ctx* ctx, const char* const* field_names, const siz
     struct TsFrame { uint64_t block; uint32_t frame; uint64_t rel; };
     std::vector<TsFrame> ts_frames;
     if (mode != UP_HEADERS) {
-        uint64_t zc = collect_values_blocks(blocks, nblocks, zv, mode == UP_VALUES ? need : nullptr, nfields);
+        uint64_t zc = collect_values_blocks(blocks, nblocks, zv, values_phase ? need : nullptr, nfields);
         for (const ZValuesBlock& v : zv) if (v.n) zpieces.push_back({v.p, v.n, v.zoff});
-        // ZSTD-compressed timestamps blocks (marshal types 1 and 4) travel the same way, behind the values blocks
-        for (uint64_t b = 0; b < nblocks; b++) {
+        // ZSTD-compressed timestamps blocks (marshal types 1 and 4) travel the same way, behind the values blocks (a late call stages none)
+        for (uint64_t b = 0; b < nblocks && mode != UP_LATE; b++) {
             const vlscan_block& blk = blocks[b];
             if (blk.ts_marshal_type != MT_ZSTD_NEAREST_DELTA2 && blk.ts_marshal_type != MT_ZSTD_NEAREST_DELTA) continue;
             if (blk.timestamps_len > vl::part::kMaxTimestampsBlockSize) throw BadInput("timestamps block size cannot exceed 8 MiB");   // getTimestamps block_search.go:490-493
@@ -402,7 +408,7 @@ static void do_upload(vlscan_ctx* ctx, const char* const* field_names, const siz
         const vlscan_block& blk = blocks[b];
         if (blk.rows > (8u << 20)) throw BadInput("block rows exceed maxRowsPerBlock (8Mi)");   // consts.go:24
         rows[b] = (uint32_t)blk.rows;
-        if (blk.ts_marshal_type && mode != UP_HEADERS) {   // the timestamps column: encoded deltas as stored + timestampsHeader (block_header.go:990-997)
+        if (blk.ts_marshal_type && (mode == UP_FULL || mode == UP_VALUES)) {   // the timestamps column: encoded deltas as stored + timestampsHeader (block_header.go:990-997)
             if (blk.ts_marshal_type > MT_NEAREST_DELTA) throw BadInput("unknown MarshalType of a timestamps block");
             if (blk.timestamps_len > vl::part::kMaxTimestampsBlockSize) throw BadInput("timestamps block size cannot exceed 8 MiB");
             if (tsv.empty()) { tsv.resize(nblocks); memset(tsv.data(), 0, nblocks * sizeof(DevTimestamps)); }
@@ -426,11 +432,12 @@ static void do_upload(vlscan_ctx* ctx, const char* const* field_names, const siz
             const vlscan_column& c = blk.cols[k];
             if (c.field >= nfields) throw BadInput("column refers to a field outside the batch field table");
             DevColumn& d = cols[(size_t)b * nfields + c.field];
-            if (mode == UP_VALUES) {   // the headers are on the device since phase 1; now the values of the columns the probe pass marked
+            if (values_phase) {   // the headers are on the device since phase 1; now the values of the columns the probe pass (or the caller) marked
                 if (c.kind != VLSCAN_COL_VALUES) continue;
-                if (!need[b * nfields + c.field]) { d.values_state = VALUES_ABSENT; continue; }
+                if (!need[b * nfields + c.field]) { if (mode == UP_VALUES) d.values_state = VALUES_ABSENT; continue; }
                 d.values_state = VALUES_STAGED;
                 stage_values(blk, c, d, b);
+                if (mode == UP_LATE) late_cells.push_back((uint64_t)b * nfields + c.field);
                 continue;
             }
             if (d.kind != COL_MISSING) throw BadInput("duplicate column for one field in a block");
@@ -476,11 +483,25 @@ static void do_upload(vlscan_ctx* ctx, const char* const* field_names, const siz
     for (const TsFrame& tf : ts_frames) { tsv[tf.block].off = regen_base + tf.rel; zjob.set_dst(tf.frame, regen_base + tf.rel); }
     if (!ondisk.empty() || !ts_frames.empty()) cursor = regen_base + regen_cursor;
     const uint64_t arena_bytes = cursor + kArenaPad;
-    (mode == UP_HEADERS ? out->harena_bytes : out->arena_bytes) = arena_bytes;
+    if (mode != UP_LATE) (mode == UP_HEADERS ? out->harena_bytes : out->arena_bytes) = arena_bytes;
     if (mode == UP_FULL) out->harena_bytes = 0;
     t_desc = now();
     arena_buf.ensure(arena_bytes);
     t_alloc = now();
+    // Late cells keep the arena-relative addressing of every kernel: their offsets are taken from the batch arena's base to the late region
+    // (modulo 2^64, so a region below the arena works too), and k_finish_ondisk_cols reads them against that base as well.
+    uint8_t* cols_base = arena_buf.as<uint8_t>();
+    std::vector<ColPatch> patches;
+    if (mode == UP_LATE) {
+        const uint64_t delta = (uint64_t)(uintptr_t)arena_buf.p - (uint64_t)(uintptr_t)out->arena.p;
+        cols_base = out->arena.as<uint8_t>();
+        patches.resize(late_cells.size());
+        for (size_t i = 0; i < late_cells.size(); i++) {
+            DevColumn& d = cols[late_cells[i]];
+            d.lens_off += delta; d.data_off += delta;
+            patches[i].col = late_cells[i]; patches[i].c = d;
+        }
+    }
     // the arena is cleared on the compute stream; the copy stream takes over from there
     cudaEvent_t ev_cleared = events.make(), ev_copied = events.make();
     VL_CUDA(cudaMemsetAsync(arena_buf.p, 0, arena_bytes, ctx->stream));
@@ -502,16 +523,27 @@ static void do_upload(vlscan_ctx* ctx, const char* const* field_names, const siz
         if (dbg) t_zrun = now();
     }
     copy_pieces(pieces, arena_buf.as<uint8_t>());
-    out->cols.ensure(std::max<size_t>(cols.size() * sizeof(DevColumn), 16));
-    if (!cols.empty()) VL_CUDA(cudaMemcpyAsync(out->cols.p, cols.data(), cols.size() * sizeof(DevColumn), cudaMemcpyHostToDevice, cs));
-    if (mode != UP_HEADERS) out->has_ts = any_ts; else out->has_ts = false;
+    if (mode == UP_LATE) {   // only the entries of the cells staged here: the table on the device has what k_finish_ondisk_cols derived since
+        ctx->patch.ensure(std::max<size_t>(patches.size() * sizeof(ColPatch), 16));
+        if (!patches.empty()) VL_CUDA(cudaMemcpyAsync(ctx->patch.p, patches.data(), patches.size() * sizeof(ColPatch), cudaMemcpyHostToDevice, cs));
+        h2d += patches.size() * sizeof(ColPatch);
+    } else {
+        out->cols.ensure(std::max<size_t>(cols.size() * sizeof(DevColumn), 16));
+        if (!cols.empty()) VL_CUDA(cudaMemcpyAsync(out->cols.p, cols.data(), cols.size() * sizeof(DevColumn), cudaMemcpyHostToDevice, cs));
+        h2d += cols.size() * sizeof(DevColumn);
+    }
+    if (mode == UP_FULL || mode == UP_VALUES) out->has_ts = any_ts; else if (mode == UP_HEADERS) out->has_ts = false;
     if (any_ts) {
         out->ts.ensure(nblocks * sizeof(DevTimestamps));
         VL_CUDA(cudaMemcpyAsync(out->ts.p, tsv.data(), nblocks * sizeof(DevTimestamps), cudaMemcpyHostToDevice, cs));
         h2d += nblocks * sizeof(DevTimestamps);
     }
     VL_CUDA(cudaEventRecord(ev_copied, cs));
-    h2d += cols.size() * sizeof(DevColumn);
+    if (!patches.empty()) {
+        VL_CUDA(cudaStreamWaitEvent(ctx->stream, ev_copied, 0));
+        k_patch_cols<<<cdiv(patches.size(), 128), 128, 0, ctx->stream>>>(out->cols.as<DevColumn>(), ctx->patch.as<ColPatch>(), (uint32_t)patches.size());
+        launch_check(ctx);
+    }
     const double t_enq = dbg ? now() : 0;
     if (have_z) {
         // the on-disk payloads are being regenerated in HBM; derive lens_type / lens_const / data_const from the regenerated lens blocks
@@ -520,7 +552,7 @@ static void do_upload(vlscan_ctx* ctx, const char* const* field_names, const siz
         VL_CUDA(cudaMemsetAsync(ctx->zcols.p, 0, 16, ctx->stream));
         VL_CUDA(cudaMemcpyAsync(ctx->zcols.as<uint8_t>() + 16, ocols.data(), ocols.size() * sizeof(OndiskCol), cudaMemcpyHostToDevice, ctx->stream));
         if (!ocols.empty()) {
-            k_finish_ondisk_cols<<<cdiv(ocols.size(), 128), 128, 0, ctx->stream>>>(arena_buf.as<uint8_t>(), out->cols.as<DevColumn>(), (const OndiskCol*)(ctx->zcols.as<uint8_t>() + 16),
+            k_finish_ondisk_cols<<<cdiv(ocols.size(), 128), 128, 0, ctx->stream>>>(cols_base, out->cols.as<DevColumn>(), (const OndiskCol*)(ctx->zcols.as<uint8_t>() + 16),
                                                                                      (uint32_t)ocols.size(), ctx->zcols.as<unsigned long long>());
             launch_check(ctx);
         }
@@ -534,15 +566,17 @@ static void do_upload(vlscan_ctx* ctx, const char* const* field_names, const siz
     VL_CUDA(cudaStreamWaitEvent(ctx->stream, ev_copied, 0));
     if (dbg) { VL_CUDA(cudaStreamSynchronize(ctx->stream)); t_copy = now(); }
     if (nfields) out->note_columns(cols);
-    if (mode != UP_VALUES) finish_batch_layout(ctx, out, rows);   // synchronises the stream => `owned`, `cols`, staging are safe to drop
-    else VL_CUDA(cudaStreamSynchronize(ctx->stream));             // the layout tables are there since the header phase
+    if (!values_phase) finish_batch_layout(ctx, out, rows);   // synchronises the stream => `owned`, `cols`, staging are safe to drop
+    else VL_CUDA(cudaStreamSynchronize(ctx->stream));         // the layout tables are there since the header phase
     if (dbg) fprintf(stderr, "[vlscan upload] blocks=%llu arena=%.1f MB h2d=%.1f MB pieces=%zu+%zu pinned=%d: describe %.1f ms, alloc %.1f ms, copy %.1f ms (%.1f GB/s), "
                              "zstd %llu frames / %llu blocks / %llu sequences: enqueue %.1f ms, decode %.1f ms; layout %.1f ms\n", (unsigned long long)nblocks,
                      arena_bytes / 1e6, h2d / 1e6, pieces.size(), zpieces.size(), (int)all_pinned, 1e3 * (t_desc - t_start), 1e3 * (t_alloc - t_desc), 1e3 * (t_enq - (t_zrun > 0 ? t_zrun : t_h2d)), h2d / 1e9 / std::max(t_copy - t_start, 1e-9),
                      (unsigned long long)zjob.frames(), (unsigned long long)zjob.compressed_blocks(), (unsigned long long)zjob.sequences(), 1e3 * (t_zrun > 0 ? t_zrun - t_h2d : 0), 1e3 * (t_copy - t_enq), 1e3 * (now() - t_copy));
     (void)all_pinned;
-    if (mode != UP_VALUES) h2d += out->nwords * 12 + nblocks * 12;
+    if (!values_phase) h2d += out->nwords * 12 + nblocks * 12;
     if (mode == UP_FULL) std::vector<DevColumn>().swap(out->h_cols);   // only a bloom-first upload needs the table again
+    if (mode == UP_LATE) out->late_used++;
+    if (zframes) *zframes += zjob.frames();
     if (stats) stats->h2d_bytes += h2d;
 }
 
@@ -760,7 +794,7 @@ static void do_scan(vlscan_ctx* ctx, const vlscan_program* prog, const vlscan_ba
         launch_check(ctx);
     }
     VL_CUDA(cudaEventRecord(ctx->ev_end, ctx->stream));
-    ctx->last_batch = batch; ctx->has_result = true; ctx->last_launches = ctx->launches - launches0;
+    ctx->last_batch = batch; ctx->has_result = true; ctx->kept = false; ctx->last_launches = ctx->launches - launches0;
     ctx->last_nblocks = batch->nblocks; ctx->last_nwords = batch->nwords; ctx->last_rows = batch->rows;
     if (stats) {
         read_stats(ctx, stats, true);
@@ -833,7 +867,7 @@ void vlscan_ctx_free(vlscan_ctx* ctx) {
     for (auto& r : ctx->row_off8) r.release();
     for (auto& r : ctx->ready) r.release();
     ctx->zsrc.release(); ctx->zcols.release(); ctx->ztest.release(); ctx->ts_vals.release();
-    for (DevBuf* b : {&ctx->hit_block, &ctx->glens, &ctx->goffs, &ctx->gtiles, &ctx->gout, &ctx->gstat, &ctx->hblk, &ctx->htab, &ctx->hgrp, &ctx->lcand, &ctx->ftab}) b->release();
+    for (DevBuf* b : {&ctx->hit_block, &ctx->glens, &ctx->goffs, &ctx->gtiles, &ctx->gout, &ctx->gstat, &ctx->hblk, &ctx->htab, &ctx->hgrp, &ctx->lcand, &ctx->ftab, &ctx->patch, &ctx->unstaged}) b->release();
     for (DevBuf& b : ctx->ftxt) b.release();
     zstd_dev_free(ctx->zdev);
     delete ctx->pool;
@@ -1306,7 +1340,8 @@ static void check_gather_errors(vlscan_ctx* ctx) {
     VL_CUDA(cudaMemcpyAsync(h, ctx->gstat.p, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
     VL_CUDA(cudaStreamSynchronize(ctx->stream));
     static const char* const msg[] = {"", "cannot unmarshal strings: row lengths do not add up to the data length", "too big index for dict value", "unexpected length for binary representation of a number", "",
-                                      "unexpected uint64 block type", "the timestamps of a block with selected rows were not handed over", "cannot unmarshal timestamps", "",
+                                      "unexpected uint64 block type", "the timestamps of a block with selected rows were not handed over", "cannot unmarshal timestamps",
+                                      "the values of a cell with selected rows are not on the device (vlscan_stage_selected stages them)",
                                       "the decoded timestamps of a block contradict the minimum / maximum of its header"};
     if (h[ST_ERROR]) throw BadInput(msg[std::min<unsigned long long>(h[ST_ERROR], 9)]);
 }
@@ -1337,10 +1372,21 @@ static int field_slot(const vlscan_batch* b, const std::string& name) {
     return -1;
 }
 // row offsets of the strings blocks with hits in column `slot` (kept from the scan where it already computed them); `with_rows` (default: the
-// scan's counts) != 0 marks the blocks whose offsets are needed
-static const uint32_t* hit_row_offsets(vlscan_ctx* ctx, int slot, const uint32_t* with_rows = nullptr) {
+// scan's counts) != 0 marks the blocks whose offsets are needed.  On a kept batch every such block must have the field's values on the
+// device: the call fails naming the field otherwise (the kernels would report ERR_VALUES_ABSENT, which cannot say which field it was).
+static const uint32_t* hit_row_offsets(vlscan_ctx* ctx, int slot, const std::string& name, const uint32_t* with_rows = nullptr) {
     if (slot < 0) return nullptr;
     BatchView B = ctx->last_batch->view();
+    if (ctx->last_batch->split_hdr && B.nblocks) {   // only a bloom-first / kept staging leaves values on the host
+        ctx->unstaged.ensure(16);
+        VL_CUDA(cudaMemsetAsync(ctx->unstaged.p, 0, 8, ctx->stream));
+        k_unstaged_count<<<cdiv(B.nblocks, 256), 256, 0, ctx->stream>>>(B, with_rows ? with_rows : ctx->counts.as<uint32_t>(), slot, ctx->unstaged.as<unsigned long long>());
+        launch_check(ctx);
+        unsigned long long n = 0;
+        VL_CUDA(cudaMemcpyAsync(&n, ctx->unstaged.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaStreamSynchronize(ctx->stream));
+        if (n) throw BadInput("field `" + name + "`: its values are not on the device in " + std::to_string(n) + " block(s) with selected rows (stage them with vlscan_stage_selected)");
+    }
     uint32_t* wc = ctx->work_count.as<uint32_t>();
     VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
     k_hit_blocks_list<<<cdiv(B.nblocks, 256), 256, 0, ctx->stream>>>(B, with_rows ? with_rows : ctx->counts.as<uint32_t>(), slot, 0, ctx->lens_blocks.as<uint32_t>(), wc); launch_check(ctx);
@@ -1380,7 +1426,7 @@ int vlscan_gather_values(vlscan_ctx* ctx, const char* field, size_t field_len, u
         if (!n) return;
         std::string name(field, field_len); if (name.empty()) name = "_msg";   // getCanonicalColumnName
         const int slot = field_slot(ctx->last_batch, name);
-        const uint32_t* ro = hit_row_offsets(ctx, slot);
+        const uint32_t* ro = hit_row_offsets(ctx, slot, name);
         const uint32_t* rows = ctx->hits.as<uint32_t>(); const uint32_t* blocks = ctx->hit_block.as<uint32_t>();
         const uint64_t total = text_offsets(ctx, slot, ro, rows, blocks, n);
         if (out_total_bytes) *out_total_bytes = total;
@@ -1420,7 +1466,7 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
         HitsQuery hq;
         memset(&hq, 0, sizeof hq);
         hq.step = q->step; hq.offset = q->offset; hq.calendar = q->calendar; hq.nby = q->nby;
-        for (uint32_t f = 0; f < q->nby; f++) { hq.slot[f] = field_slot(b, names[f]); hq.row_off8[f] = hit_row_offsets(ctx, hq.slot[f]); }
+        for (uint32_t f = 0; f < q->nby; f++) { hq.slot[f] = field_slot(b, names[f]); hq.row_off8[f] = hit_row_offsets(ctx, hq.slot[f], names[f]); }
         // buckets of the blocks; timestamps decoded only where a block spans several buckets
         unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
         uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* row_blocks = ctx->row_blocks.as<uint32_t>();
@@ -1608,7 +1654,7 @@ int vlscan_last_rows(vlscan_ctx* ctx, const vlscan_last_query* q, int64_t* out_t
         uint64_t value_bytes = 0;
         for (uint32_t f = 0; f < q->nfields && n; f++) {
             const int slot = field_slot(b, names[f]);
-            const uint32_t* ro = hit_row_offsets(ctx, slot, blk_mark);
+            const uint32_t* ro = hit_row_offsets(ctx, slot, names[f], blk_mark);
             const uint64_t total = text_offsets(ctx, slot, ro, sel_row, sel_blk, n);
             value_bytes += total;
             toffs[f].resize(n + 1); tbytes[f].resize(total);
@@ -1716,7 +1762,7 @@ int vlscan_facets(vlscan_ctx* ctx, const vlscan_facets_query* q, uint8_t* out_dr
                 FacetField& F = hf[f];
                 F.is_time = names[f] == "_time";
                 F.slot = F.is_time ? -1 : field_slot(b, names[f]);
-                F.row_off8 = hit_row_offsets(ctx, F.slot);
+                F.row_off8 = hit_row_offsets(ctx, F.slot, names[f]);
                 F.toffs = nullptr; F.tbytes = nullptr;
                 has_time |= F.is_time;
                 if (F.slot < 0 || !nblk) continue;
@@ -1895,8 +1941,19 @@ int vlscan_result_device_ptrs(vlscan_ctx* ctx, void** bitmap_words, void** match
     return 0;
 }
 
-int vlscan_scan_batch(vlscan_ctx* ctx, const vlscan_program* prog, const char* const* field_names, const size_t* field_name_lens, uint32_t nfields,
-                      const vlscan_block* blocks, uint64_t nblocks, uint64_t* out_bitmap_words, uint32_t* out_match_counts, vlscan_stats* stats) {
+// what vlscan_stage_selected checks a values column's descriptor against: its stage and payload lengths
+static vlscan_batch::CellSig cell_sig(const vlscan_column& c) {
+    vlscan_batch::CellSig g;
+    g.stage = c.stage;
+    if (c.stage == VLSCAN_STAGE_ONDISK) g.len0 = c.values_len; else { g.len0 = c.lens_items_len; g.len1 = c.data_len; }
+    return g;
+}
+
+// The body of vlscan_scan_batch and vlscan_scan_batch_keep.  keep = false is vlscan_scan_batch as it always was.  keep = true always stages in two
+// phases (UP_HEADERS, then UP_VALUES with a `need` mask): the probe pass decides the values of the program's fields when it runs, else all of
+// them are marked; cells of the other fields (output fields) keep their values on the host.  The batch then stays the ctx's last result.
+static int scan_batch_impl(vlscan_ctx* ctx, const vlscan_program* prog, const char* const* field_names, const size_t* field_name_lens, uint32_t nfields,
+                           const vlscan_block* blocks, uint64_t nblocks, uint64_t* out_bitmap_words, uint32_t* out_match_counts, vlscan_stats* stats, bool keep) {
     // the staging batch (HBM arena + descriptor tables) is recycled across calls of this ctx: a search worker submits batch after
     // batch, so cudaMalloc / cudaFree of a multi-GB arena per call would sit on the critical path
     vlscan_batch* b = ctx->recycle ? ctx->recycle : new vlscan_batch();
@@ -1904,13 +1961,14 @@ int vlscan_scan_batch(vlscan_ctx* ctx, const vlscan_program* prog, const char* c
     b->field_names.clear(); b->slot_vt_mask.clear();
     uint64_t launches0 = ctx->launches;
     // which fields' bloom filters the program can ever probe: leaves with token hashes (or in() / contains_any() token sets) and the per-field
-    // tokens of the AND / OR pre-passes
-    std::vector<char> need_bloom(nfields, 0);
+    // tokens of the AND / OR pre-passes; and (keep) which batch fields the program references at all
+    std::vector<char> need_bloom(nfields, 0), in_prog(nfields, 0);
     {
         const Program& P = prog->p;
-        auto mark = [&](int field) { for (uint32_t s = 0; s < nfields; s++) if (std::string(field_names[s], field_name_lens[s]) == P.fields[field]) need_bloom[s] = 1; };
-        for (const DevLeaf& L : P.leaves) if (L.nhashes || L.nhashes2 || L.in_nsets) mark(L.field);
-        for (const DevPrepass& pp : P.prepass) if (pp.nhashes) mark(pp.field);
+        auto mark = [&](std::vector<char>& m, int field) { for (uint32_t s = 0; s < nfields; s++) if (std::string(field_names[s], field_name_lens[s]) == P.fields[field]) m[s] = 1; };
+        for (const DevLeaf& L : P.leaves) if (L.nhashes || L.nhashes2 || L.in_nsets) mark(need_bloom, L.field);
+        for (const DevPrepass& pp : P.prepass) if (pp.nhashes) mark(need_bloom, pp.field);
+        if (keep) for (size_t f = 0; f < P.fields.size(); f++) mark(in_prog, (int)f);
     }
     // Bloom-first staging (the reference reads a column's values only after the block got past the bloom filters, block_search.go:411-474): when
     // the program probes bloom filters at all, the headers and bloom filters go first, a probe pass marks the columns some filter can reach,
@@ -1922,26 +1980,46 @@ int vlscan_scan_batch(vlscan_ctx* ctx, const vlscan_program* prog, const char* c
     bool probes = false;
     for (char c : need_bloom) probes |= c != 0;
     if (ctx->bf_prog != (const void*)prog) { ctx->bf_prog = prog; ctx->bf_skip = 0; }
-    const bool two_phase = bf != 0 && probes && nblocks > 0 && (bf == 2 || ctx->bf_skip == 0);
-    if (!two_phase && ctx->bf_skip > 0) ctx->bf_skip--;
+    const bool probe = bf != 0 && probes && nblocks > 0 && (bf == 2 || ctx->bf_skip == 0);
+    if (!probe && ctx->bf_skip > 0) ctx->bf_skip--;
     int rc;
-    if (two_phase) {
+    if (probe || keep) {
         rc = guarded(ctx, [&] {
             do_upload(ctx, field_names, field_name_lens, nfields, blocks, nblocks, b, stats, &need_bloom, UP_HEADERS);
             std::vector<uint8_t> need;
-            do_probe(ctx, prog, b, need);
+            if (probe) do_probe(ctx, prog, b, need);
+            else {   // keep without a probe: every values cell of the program's own fields
+                need.assign(std::max<size_t>((size_t)nblocks * nfields, 1), 0);   // never empty: the values phase needs a mask, also for no block or no field
+                for (uint64_t i = 0; i < nblocks; i++)
+                    for (uint32_t k = 0; k < blocks[i].ncols; k++) if (blocks[i].cols[k].field < nfields && in_prog[blocks[i].cols[k].field]) need[i * nfields + blocks[i].cols[k].field] = 1;
+            }
+            // the adaptive rule weighs what the probe saved on the fields it can prune: with keep, the program's fields only
             uint64_t vals_all = 0, vals_need = 0, cols_all = 0, cols_need = 0;
             for (uint64_t i = 0; i < nblocks; i++)
                 for (uint32_t k = 0; k < blocks[i].ncols; k++) {
                     const vlscan_column& c = blocks[i].cols[k];
                     if (c.kind != VLSCAN_COL_VALUES || c.field >= nfields) continue;
+                    const bool needed = need[i * nfields + c.field] != 0;
+                    cols_all++; cols_need += needed;
+                    if (keep && !in_prog[c.field]) continue;
                     const uint64_t n = c.stage == VLSCAN_STAGE_ONDISK ? c.values_len : c.lens_items_len + c.data_len;
-                    vals_all += n; cols_all++;
-                    if (need[i * nfields + c.field]) { vals_need += n; cols_need++; }
+                    vals_all += n;
+                    if (needed) vals_need += n;
                 }
-            if (stats) { stats->staged_columns += cols_need; stats->pruned_columns += cols_all - cols_need; }
-            if (vals_need * 8 > vals_all * 7) ctx->bf_skip = 7;
+            if (stats && probe) { stats->staged_columns += cols_need; stats->pruned_columns += cols_all - cols_need; }   // as vlscan_scan_batch: 0 / 0 without a probe
+            if (probe && vals_need * 8 > vals_all * 7) ctx->bf_skip = 7;
             do_upload(ctx, field_names, field_name_lens, nfields, blocks, nblocks, b, stats, &need_bloom, UP_VALUES, need.data());
+            if (keep) {   // what vlscan_stage_selected checks its descriptors against
+                b->h_sig.assign((size_t)nblocks * nfields, vlscan_batch::CellSig{});
+                b->h_ncols.resize(nblocks);
+                for (uint64_t i = 0; i < nblocks; i++) {
+                    b->h_ncols[i] = blocks[i].ncols;
+                    for (uint32_t k = 0; k < blocks[i].ncols; k++) {
+                        const vlscan_column& c = blocks[i].cols[k];
+                        if (c.kind == VLSCAN_COL_VALUES) b->h_sig[i * nfields + c.field] = cell_sig(c);
+                    }
+                }
+            }
         });
     } else rc = guarded(ctx, [&] { do_upload(ctx, field_names, field_name_lens, nfields, blocks, nblocks, b, stats, &need_bloom); });
     if (rc) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamSynchronize(ctx->stream); }   // nothing may still read the caller's buffers
@@ -1950,8 +2028,100 @@ int vlscan_scan_batch(vlscan_ctx* ctx, const vlscan_program* prog, const char* c
     if (!rc && stats) {
         rc = guarded(ctx, [&] { read_stats(ctx, stats, true); stats->blocks += b->nblocks; stats->rows += b->rows; stats->gpu_launches += ctx->launches - launches0; });
     }
-    ctx->has_result = false; ctx->last_batch = nullptr;
+    if (keep && !rc) ctx->kept = true;   // the result of vlscan_scan_resident above stays, on the batch it staged
+    else { ctx->has_result = false; ctx->last_batch = nullptr; ctx->kept = false; }
     ctx->recycle = b;
+    return rc;
+}
+
+int vlscan_scan_batch(vlscan_ctx* ctx, const vlscan_program* prog, const char* const* field_names, const size_t* field_name_lens, uint32_t nfields,
+                      const vlscan_block* blocks, uint64_t nblocks, uint64_t* out_bitmap_words, uint32_t* out_match_counts, vlscan_stats* stats) {
+    return scan_batch_impl(ctx, prog, field_names, field_name_lens, nfields, blocks, nblocks, out_bitmap_words, out_match_counts, stats, false);
+}
+
+int vlscan_scan_batch_keep(vlscan_ctx* ctx, const vlscan_program* prog, const char* const* field_names, const size_t* field_name_lens, uint32_t nfields,
+                           const vlscan_block* blocks, uint64_t nblocks, uint64_t* out_bitmap_words, uint32_t* out_match_counts, vlscan_stats* stats) {
+    if (!ctx || !prog) return guarded(nullptr, [&] { throw BadInput(!ctx ? "vlscan_scan_batch_keep needs a vlscan_ctx on a CUDA device (there is no CPU fallback)" : "vlscan_scan_batch_keep: no program"); });
+    return scan_batch_impl(ctx, prog, field_names, field_name_lens, nfields, blocks, nblocks, out_bitmap_words, out_match_counts, stats, true);
+}
+
+int vlscan_stage_selected(vlscan_ctx* ctx, const vlscan_block* blocks, uint64_t nblocks, const char* const* field_names, const size_t* field_name_lens, uint32_t nfields,
+                          const uint32_t* block_list, uint64_t nlist, uint64_t out_info[4]) {
+    uint64_t info[4] = {0, 0, 0, 0};   // cells staged, cells already staged, H2D bytes, frames through the device decoder
+    bool staging = false;
+    const int rc = guarded(ctx, [&] {
+        if (nfields == 0) throw BadInput("vlscan_stage_selected needs at least one field");
+        if (!field_names || !field_name_lens) throw BadInput("vlscan_stage_selected: field names missing");
+        if (nlist && !block_list) throw BadInput("vlscan_stage_selected: block list missing");
+        if (!ctx) throw BadInput("vlscan_stage_selected needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
+        if (!ctx->has_result || !ctx->kept || !ctx->recycle || ctx->last_batch != ctx->recycle) throw BadInput("no kept scan on this ctx (vlscan_scan_batch_keep keeps one until the next scan)");
+        vlscan_batch* b = ctx->recycle;
+        VL_CUDA(cudaSetDevice(ctx->device));
+        const uint32_t nf = b->nfields;
+        std::vector<char> want(nf, 0);
+        for (uint32_t f = 0; f < nfields; f++) {
+            std::string n(field_names[f], field_name_lens[f]);
+            if (n.empty()) n = "_msg";   // getCanonicalColumnName
+            const int slot = field_slot(b, n);
+            if (slot < 0) throw BadInput("field `" + n + "` is not a field of the kept batch");
+            want[slot] = 1;
+        }
+        if (!blocks || nblocks != b->nblocks) throw BadInput("the block descriptors differ from those of the kept scan: " + std::to_string(nblocks) + " blocks instead of " + std::to_string(b->nblocks));
+        std::vector<uint8_t> sel(nblocks, 0);
+        if (block_list) {
+            for (uint64_t i = 0; i < nlist; i++) {
+                if (block_list[i] >= nblocks) throw BadInput("block_list[" + std::to_string(i) + "] = " + std::to_string(block_list[i]) + " is outside the kept batch of " + std::to_string(nblocks) + " blocks");
+                sel[block_list[i]] = 1;
+            }
+        } else if (nblocks) {   // every block with selected rows
+            std::vector<uint32_t> cnt(nblocks);
+            VL_CUDA(cudaMemcpyAsync(cnt.data(), ctx->counts.p, nblocks * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaStreamSynchronize(ctx->stream));
+            for (uint64_t i = 0; i < nblocks; i++) sel[i] = cnt[i] != 0;
+        }
+        // the descriptors of the blocks this call reads must be the ones the keep call staged from
+        auto mismatch = [&](uint64_t i, const char* what) { return BadInput("the block descriptors differ from those of the kept scan: block " + std::to_string(i) + ", " + what); };
+        for (uint64_t i = 0; i < nblocks; i++) {
+            if (!sel[i]) continue;
+            const vlscan_block& blk = blocks[i];
+            if (blk.rows != b->h_rows[i]) throw mismatch(i, "row count");
+            if (blk.ncols != b->h_ncols[i] || (blk.ncols && !blk.cols)) throw mismatch(i, "column count");
+            for (uint32_t k = 0; k < blk.ncols; k++) {
+                const vlscan_column& c = blk.cols[k];
+                if (c.field >= nf) throw mismatch(i, "field of a column");
+                const DevColumn& d = b->h_cols[i * nf + c.field];
+                if (c.kind == VLSCAN_COL_CONST) { if (d.kind != COL_CONST || d.meta_len != c.const_len) throw mismatch(i, "const column"); }
+                else if (c.kind == VLSCAN_COL_VALUES) {
+                    if (d.kind != COL_VALUES || d.vt != c.value_type) throw mismatch(i, "column kind or value type");
+                    const vlscan_batch::CellSig want = cell_sig(c), &had = b->h_sig[i * nf + c.field];
+                    if (had.stage != want.stage || had.len0 != want.len0 || had.len1 != want.len1) throw mismatch(i, "values stage or payload lengths");
+                } else throw mismatch(i, "column kind");
+            }
+        }
+        // const, dict tables and absent cells are on the device (or nothing) already; values cells whose payload the keep call left on the host are staged
+        std::vector<uint8_t> need((size_t)nblocks * nf, 0);
+        for (uint64_t i = 0; i < nblocks; i++) {
+            if (!sel[i]) continue;
+            for (uint32_t s = 0; s < nf; s++) {
+                const DevColumn& d = b->h_cols[i * nf + s];
+                if (!want[s] || d.kind != COL_VALUES) continue;
+                if (d.values_state == VALUES_STAGED) info[1]++;
+                else { need[i * nf + s] = 1; info[0]++; }
+            }
+        }
+        if (!info[0]) return;
+        vlscan_stats st;
+        memset(&st, 0, sizeof st);
+        staging = true;
+        do_upload(ctx, nullptr, nullptr, nf, blocks, nblocks, b, &st, nullptr, UP_LATE, need.data(), &info[3]);
+        info[2] = st.h2d_bytes;
+    });
+    if (rc && staging) {   // a half-staged batch is not a result any more; nothing may still read the caller's buffers
+        cudaStreamSynchronize(ctx->copy_stream); cudaStreamSynchronize(ctx->stream);
+        ctx->has_result = false; ctx->last_batch = nullptr; ctx->kept = false;
+        info[0] = info[1] = info[2] = info[3] = 0;
+    }
+    if (out_info && !rc) memcpy(out_info, info, sizeof info);
     return rc;
 }
 

@@ -62,6 +62,13 @@ struct vlscan_batch {
     std::vector<uint32_t> h_rows;
     std::vector<uint64_t> h_word_off;
     std::vector<uint32_t> slot_vt_mask;   // per field slot: bit vt set when some block stores the field with that valueType
+    // kept batches (vlscan_scan_batch_keep) only:
+    std::vector<vl::DevBuf> late;         // one region per vlscan_stage_selected call; late cells address it by an offset from `arena` (DESIGN §3.12)
+    size_t late_used = 0;                 // regions holding payloads of the current batch (the others are reused by later calls; there are as many
+                                          // regions as stage calls one kept batch ever received, each at its largest size, until the batch is freed)
+    struct CellSig { uint64_t len0 = 0, len1 = 0; uint32_t stage = 0; };   // a values column: ONDISK (values_len, 0), DECODED (lens_items_len, data_len)
+    std::vector<CellSig> h_sig;           // per (block, field) cell, as the keep call was given it
+    std::vector<uint32_t> h_ncols;        // per block: the number of columns it was described with
     void note_columns(const std::vector<vl::DevColumn>& cols) {
         slot_vt_mask.assign(nfields, 0);
         for (size_t i = 0; i < cols.size(); i++) if (cols[i].kind == vl::COL_VALUES) slot_vt_mask[i % nfields] |= 1u << cols[i].vt;
@@ -74,8 +81,15 @@ struct vlscan_batch {
         v.nblocks = (uint32_t)nblocks; v.nfields = nfields; v.nwords = nwords;
         return v;
     }
-    uint64_t device_bytes() const { return arena.cap + harena.cap + cols.cap + blk_rows.cap + blk_word_off.cap + word_block.cap + init_bitmap.cap + ts.cap; }
-    ~vlscan_batch() { cudaSetDevice(device); arena.release(); harena.release(); cols.release(); blk_rows.release(); blk_word_off.release(); word_block.release(); init_bitmap.release(); ts.release(); }
+    uint64_t device_bytes() const {
+        uint64_t n = arena.cap + harena.cap + cols.cap + blk_rows.cap + blk_word_off.cap + word_block.cap + init_bitmap.cap + ts.cap;
+        for (const vl::DevBuf& r : late) n += r.cap;
+        return n;
+    }
+    ~vlscan_batch() {
+        cudaSetDevice(device); arena.release(); harena.release(); cols.release(); blk_rows.release(); blk_word_off.release(); word_block.release(); init_bitmap.release(); ts.release();
+        for (vl::DevBuf& r : late) r.release();
+    }
 };
 
 struct vlscan_ctx {
@@ -108,7 +122,9 @@ struct vlscan_ctx {
     // last scan
     const vlscan_batch* last_batch = nullptr;   // the batch of the last scan: must stay alive until its results have been fetched
     uint64_t last_nblocks = 0, last_nwords = 0, last_rows = 0;   // host-side facts about it, kept here so that counters never touch a freed batch
-    vlscan_batch* recycle = nullptr;       // staging batch reused by vlscan_scan_batch
+    vlscan_batch* recycle = nullptr;       // staging batch reused by vlscan_scan_batch and vlscan_scan_batch_keep
+    bool kept = false;                     // the last result is a kept batch (`recycle`, alive until the next scan on this ctx)
+    vl::DevBuf patch, unstaged;            // vlscan_stage_selected: the column table entries it rewrites; a counter of unstaged cells with selected rows
     bool has_result = false;
     uint64_t last_launches = 0;
     int sm_count = 132;                    // H100 SXM; vlscan_ctx_create reads the device's own count

@@ -595,6 +595,20 @@ static __global__ void k_finish_ondisk_cols(const uint8_t* __restrict__ arena, D
     }
     if (err) atomicMax(&status[0], (unsigned long long)err);
 }
+// ---- late staging of a kept batch (vlscan_stage_selected) ------------------------------------------------------------------------------
+// the column table entries of the cells staged by one call
+struct ColPatch { uint64_t col; DevColumn c; };
+static __global__ void k_patch_cols(DevColumn* __restrict__ cols, const ColPatch* __restrict__ p, uint32_t n) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) cols[p[i].col] = p[i].c;
+}
+// *count += the blocks with marks[b] != 0 whose column `slot` is a values column without its values on the device
+static __global__ void k_unstaged_count(BatchView B, const uint32_t* __restrict__ marks, int slot, unsigned long long* __restrict__ count) {
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B.nblocks || marks[b] == 0) return;
+    const DevColumn& c = B.cols[(uint64_t)b * B.nfields + slot];
+    if (c.kind == COL_VALUES && c.values_state != VALUES_STAGED) atomicAdd(count, 1ull);
+}
 
 // ---- lens decode -> byte offset of every 8th row (unmarshalUint64Items + the offsets implied by encoding.go:122-130) --------------------
 // row_off8[8 * w + g] = byte offset (within the block's data) of row 64 * (w - first word of the block) + 8 * g, for every bitmap word w of the
@@ -610,6 +624,10 @@ static __global__ void k_lens_offsets(BatchView B, int slot, const uint32_t* __r
         const uint32_t b = lens_blocks[j];
         if (ready[b]) continue;   // uniform per warp
         const DevColumn& c = B.cols[(uint64_t)b * B.nfields + slot];
+        if (c.values_state != VALUES_STAGED) {   // a kept batch's cell whose values are still on the host: never read, never marked ready
+            if (lane == 0) atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_VALUES_ABSENT);
+            continue;
+        }
         const uint32_t rows = B.blk_rows[b];
         const uint64_t w0 = B.blk_word_off[b]; const uint32_t nw = (uint32_t)(B.blk_word_off[b + 1] - w0);
         const uint8_t* lens = B.arena + c.lens_off;
@@ -1346,14 +1364,16 @@ static __global__ void k_gather_ts(BatchView B, const uint32_t* __restrict__ hit
     if (h < nhits) out[h] = (long long)ts_vals[B.blk_word_off[hit_block[h]] * 64 + hits[h]];
 }
 // The bytes of a const, strings or dict cell in row r of block b (a column of another kind: none); false for a typed column, whose text
-// must be formatted.  The decode value_text and the facets kernels share.
+// must be formatted.  The decode value_text and the facets kernels share.  A values cell whose payload is not on the device (a kept batch
+// before vlscan_stage_selected) reads as no bytes and reports ERR_VALUES_ABSENT.
 static __device__ __forceinline__ bool cell_bytes(const BatchView& B, const DevColumn& c, uint32_t b, uint32_t r, const uint32_t* __restrict__ row_off8, const uint8_t** out,
                                                   uint32_t* out_len, unsigned long long* __restrict__ stats) {
-    const uint8_t* src = nullptr; uint32_t len = 0;
+    const uint8_t* src = nullptr; uint32_t len = 0; unsigned err = ERR_NONE;   // one error report for every path
     if (c.kind == COL_CONST) { src = B.hdr + c.meta_off; len = c.meta_len; }
     else if (c.kind == COL_VALUES) {
         const uint8_t* data = B.arena + c.data_off;
-        if (c.vt == VT_STRING) {
+        if (c.values_state != VALUES_STAGED) err = ERR_VALUES_ABSENT;
+        else if (c.vt == VT_STRING) {
             if (c.data_const) { src = data; len = (uint32_t)c.data_len; }
             else if (c.lens_type >= 4) { len = c.lens_const; src = data + (uint64_t)r * len; }
             else {
@@ -1362,13 +1382,14 @@ static __device__ __forceinline__ bool cell_bytes(const BatchView& B, const DevC
                 for (uint32_t q = r & ~7u; q < r; q++) o += row_len(c, lens, q);
                 len = row_len(c, lens, r); src = data + o;
             }
-            if ((uint64_t)(src - data) + len > c.data_len) { len = 0; atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_LENS_MISMATCH); }
+            if ((uint64_t)(src - data) + len > c.data_len) { len = 0; err = ERR_LENS_MISMATCH; }
         } else if (c.vt == VT_DICT) {
             const uint32_t id = data[r];
-            if (id >= c.dict_len) atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_DICT_INDEX);
+            if (id >= c.dict_len) err = ERR_DICT_INDEX;
             else { const uint32_t* dof = (const uint32_t*)(B.hdr + c.meta_off); src = B.hdr + c.meta_off + 4 * (c.dict_len + 1) + dof[id]; len = dof[id + 1] - dof[id]; }
         } else return false;
     }
+    if (err) atomicMax(&stats[ST_ERROR], (unsigned long long)err);
     *out = src; *out_len = len;
     return true;
 }

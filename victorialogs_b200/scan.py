@@ -103,7 +103,8 @@ EXPORTS = ["vlscan_device_count", "vlscan_ctx_create", "vlscan_ctx_free", "vlsca
            "vlscan_batch_upload", "vlscan_batch_free", "vlscan_batch_nblocks", "vlscan_batch_rows", "vlscan_batch_words", "vlscan_batch_device_bytes",
            "vlscan_batch_generate", "vlscan_batch_download", "vlscan_host_blocks_get", "vlscan_host_blocks_field", "vlscan_host_blocks_bytes",
            "vlscan_host_blocks_free", "vlscan_host_blocks_compress", "vlscan_zstd_decompress", "vlscan_zstd_inspect", "vlscan_zstd_walk_digest", "vlscan_part_open", "vlscan_part_free", "vlscan_part_header", "vlscan_part_nblocks", "vlscan_part_block_header", "vlscan_part_timestamps",
-           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_truncate_timestamp", "vlscan_last_rows", "vlscan_facets", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch"]
+           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_truncate_timestamp", "vlscan_last_rows", "vlscan_facets", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch",
+           "vlscan_scan_batch_keep", "vlscan_stage_selected"]
 
 
 def lib_path():
@@ -711,6 +712,13 @@ class Batch:
             pass
 
 
+class KeptBatch:
+    """Sizes of the batch a scan_batch_keep left on the device (the library owns it; nothing to free)."""
+
+    def __init__(self, nblocks, rows, words):
+        self.nblocks, self.rows, self.words = nblocks, rows, words
+
+
 class Ctx:
     """Per search-worker context (device + stream); mirrors the per-goroutine blockSearch of storage_search.go:1041-1043."""
 
@@ -930,6 +938,34 @@ class Ctx:
         self._check(lib().vlscan_scan_batch(self.h, program.h, names, lens, C.c_uint32(len(host_blocks.field_names)), host_blocks.blocks,
                                             C.c_uint64(host_blocks.nblocks), words.ctypes.data_as(C.c_void_p), cnt.ctypes.data_as(C.c_void_p), C.byref(st)))
         return words[:nwords], cnt[:host_blocks.nblocks], st
+
+    def scan_batch_keep(self, program, host_blocks, out_words=None, out_counts=None):
+        """vlscan_scan_batch whose batch stays on the device as the ctx's last result (vlscan_scan_batch_keep): the gather and aggregation
+        calls then work on it, output fields of `host_blocks` the program does not reference are staged by stage_selected.
+        -> (words, counts, stats).  `host_blocks` must stay alive and unchanged for stage_selected."""
+        names, lens = host_blocks.name_arrays()
+        nwords = sum((r + 63) // 64 for r in host_blocks.rows)
+        words = out_words if out_words is not None else np.zeros(max(nwords, 1), dtype=np.uint64)
+        cnt = out_counts if out_counts is not None else np.zeros(max(host_blocks.nblocks, 1), dtype=np.uint32)
+        st = CStats()
+        self._last = None
+        self._check(lib().vlscan_scan_batch_keep(self.h, program.h, names, lens, C.c_uint32(len(host_blocks.field_names)), host_blocks.blocks,
+                                                 C.c_uint64(host_blocks.nblocks), words.ctypes.data_as(C.c_void_p), cnt.ctypes.data_as(C.c_void_p), C.byref(st)))
+        self._last = KeptBatch(host_blocks.nblocks, sum(host_blocks.rows), nwords)
+        return words[:nwords], cnt[:host_blocks.nblocks], st
+
+    def stage_selected(self, host_blocks, fields, blocks=None):
+        """Stage the values of `fields` of the kept batch for the blocks with selected rows, or for the block indexes in `blocks`
+        (vlscan_stage_selected).  host_blocks: the descriptors scan_batch_keep was given.
+        -> dict(staged, already_staged, h2d_bytes, frames)"""
+        names = [_b(f) for f in fields]
+        arr = (C.c_char_p * max(len(names), 1))(*names)
+        lens = (C.c_size_t * max(len(names), 1))(*[len(x) for x in names])
+        lst = None if blocks is None else np.ascontiguousarray(np.asarray(list(blocks), dtype=np.uint32))
+        out = (C.c_uint64 * 4)()
+        self._check(lib().vlscan_stage_selected(self.h, host_blocks.blocks, C.c_uint64(host_blocks.nblocks), arr, lens, C.c_uint32(len(names)),
+                                                lst.ctypes.data_as(C.c_void_p) if lst is not None else None, C.c_uint64(0 if lst is None else len(lst)), out))
+        return dict(staged=out[0], already_staged=out[1], h2d_bytes=out[2], frames=out[3])
 
     def close(self):
         if self.h:
