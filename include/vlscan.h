@@ -328,7 +328,7 @@ int vlscan_gather_values(vlscan_ctx* ctx, const char* field, size_t field_len, u
  *     /hits endpoint always: its step is a duration such as "1w").  int64 arithmetic wraps like Go's.
  *   group key: the bucket, then the text of every by-field as vlscan_gather_values yields it (typed values formatted, "" for a field a block does
  *     not have): `200` stored as uint16 in one block and as a string in another is one group.  Keys are compared byte for byte, never by hash.
- *   by_names: canonical field names ("" = _msg), at most VLSCAN_HITS_MAX_BY; "_time" is rejected.
+ *   by_names: canonical field names ("" = _msg), at most VLSCAN_HITS_MAX_BY; "_time" is rejected.  by_names and by_name_lens may be NULL only when nby == 0.
  * Output: the groups sorted by bucket, then by the key texts bytewise: out_buckets[g], out_counts[g] (rows), and the texts of group g's by-field
  * f at out_key_bytes[out_key_offsets[g * nby + f], out_key_offsets[g * nby + f + 1]) (out_key_offsets has cap_groups * nby + 1 entries).
  * out_info (may be NULL) = {groups, key bytes, selected rows, blocks whose timestamps were decoded}; it is filled also when the call fails because

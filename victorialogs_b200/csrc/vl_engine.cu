@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -101,6 +102,15 @@ ZstdWriter& zstd_writer() { static ZstdWriter z; return z; }
 
 void launch_check(vlscan_ctx* ctx) { ctx->launches++; VL_CUDA(cudaGetLastError()); }
 inline unsigned cdiv(uint64_t a, uint64_t b) { return (unsigned)((a + b - 1) / b); }
+
+// Typed arrays laid out in one scratch buffer at 16-byte alignment: take() every array, then place() grows the buffer once, sets the pointers
+// and returns the bytes laid out.
+struct Carve {
+    size_t off = 0;
+    std::vector<std::function<void(uint8_t*)>> set;
+    template <class T> Carve& take(T*& p, uint64_t n) { const size_t o = off; off += (n * sizeof(T) + 15) & ~(size_t)15; set.push_back([&p, o](uint8_t* base) { p = (T*)(base + o); }); return *this; }
+    size_t place(DevBuf& buf) { buf.ensure(std::max<size_t>(off, 16)); for (auto& f : set) f(buf.as<uint8_t>()); return off; }
+};
 
 }  // namespace
 
@@ -1295,24 +1305,6 @@ int vlscan_fetch_results(vlscan_ctx* ctx, uint64_t* out_bitmap_words, uint32_t* 
     });
 }
 
-int vlscan_fetch_hits(vlscan_ctx* ctx, uint32_t* out_hit_rows, uint64_t cap, uint64_t* out_hit_offsets) {
-    return guarded(ctx, [&] {
-        if (!ctx->has_result) throw BadInput("no scan result to fetch on this ctx");
-        VL_CUDA(cudaSetDevice(ctx->device));
-        const vlscan_batch* b = ctx->last_batch;
-        BatchView B = b->view();
-        ctx->hit_offs.ensure((b->nblocks + 1) * 8); ctx->hits.ensure(std::max<uint64_t>(cap, 4) * 4);
-        k_scan_counts<<<1, 1024, 0, ctx->stream>>>(ctx->counts.as<uint32_t>(), (uint32_t)b->nblocks, ctx->hit_offs.as<uint64_t>()); launch_check(ctx);
-        if (b->nblocks) { k_hits_compact<<<cdiv((uint64_t)b->nblocks * 32, 256), 256, 0, ctx->stream>>>(B, ctx->regs[0].as<uint64_t>(), ctx->hit_offs.as<uint64_t>(), ctx->hits.as<uint32_t>(), cap); launch_check(ctx); }
-        VL_CUDA(cudaMemcpyAsync(out_hit_offsets, ctx->hit_offs.p, (b->nblocks + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        VL_CUDA(cudaStreamSynchronize(ctx->stream));
-        uint64_t total = out_hit_offsets[b->nblocks];
-        if (total > cap) throw BadInput("hit buffer too small");
-        if (total) VL_CUDA(cudaMemcpyAsync(out_hit_rows, ctx->hits.p, total * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        VL_CUDA(cudaStreamSynchronize(ctx->stream));
-    });
-}
-
 // ---- hit materialisation ----------------------------------------------------------------------------------------------------------------------
 // hits of the last scan on the device: ctx->hits (row inside its block), ctx->hit_block, ctx->hit_offs (first hit of every block); returns their number
 static uint64_t build_hit_list(vlscan_ctx* ctx, uint64_t* out_hit_offsets) {
@@ -1321,20 +1313,32 @@ static uint64_t build_hit_list(vlscan_ctx* ctx, uint64_t* out_hit_offsets) {
     const vlscan_batch* b = ctx->last_batch;
     BatchView B = b->view();
     ctx->hit_offs.ensure((b->nblocks + 1) * 8);
-    k_scan_counts<<<1, 1024, 0, ctx->stream>>>(ctx->counts.as<uint32_t>(), (uint32_t)b->nblocks, ctx->hit_offs.as<uint64_t>()); launch_check(ctx);
+    uint64_t* offs = ctx->hit_offs.as<uint64_t>();
+    k_scan_cta<uint32_t><<<1, 1024, 0, ctx->stream>>>(ctx->counts.as<uint32_t>(), (uint32_t)b->nblocks, offs, offs + b->nblocks); launch_check(ctx);
     uint64_t total = 0;
-    VL_CUDA(cudaMemcpyAsync(&total, ctx->hit_offs.as<uint64_t>() + b->nblocks, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_hit_offsets) VL_CUDA(cudaMemcpyAsync(out_hit_offsets, ctx->hit_offs.p, (b->nblocks + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    VL_CUDA(cudaMemcpyAsync(&total, offs + b->nblocks, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_hit_offsets) VL_CUDA(cudaMemcpyAsync(out_hit_offsets, offs, (b->nblocks + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
     VL_CUDA(cudaStreamSynchronize(ctx->stream));
     ctx->hits.ensure(std::max<uint64_t>(total, 4) * 4); ctx->hit_block.ensure(std::max<uint64_t>(total, 4) * 4);
     if (b->nblocks && total) {
-        k_hits_compact2<<<cdiv((uint64_t)b->nblocks * 32, 256), 256, 0, ctx->stream>>>(B, ctx->regs[0].as<uint64_t>(), ctx->hit_offs.as<uint64_t>(), ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), total);
+        k_hits_compact<<<cdiv((uint64_t)b->nblocks * 32, 256), 256, 0, ctx->stream>>>(B, ctx->regs[0].as<uint64_t>(), offs, ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), total);
         launch_check(ctx);
     }
     ctx->gstat.ensure(ST_COUNT * 8);
     VL_CUDA(cudaMemsetAsync(ctx->gstat.p, 0, ST_COUNT * 8, ctx->stream));
     return total;
 }
+
+int vlscan_fetch_hits(vlscan_ctx* ctx, uint32_t* out_hit_rows, uint64_t cap, uint64_t* out_hit_offsets) {
+    return guarded(ctx, [&] {
+        if (!ctx->has_result) throw BadInput("no scan result to fetch on this ctx");
+        const uint64_t total = build_hit_list(ctx, out_hit_offsets);
+        if (total > cap) throw BadInput("hit buffer too small");
+        if (total) VL_CUDA(cudaMemcpyAsync(out_hit_rows, ctx->hits.p, total * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaStreamSynchronize(ctx->stream));
+    });
+}
+
 static void check_gather_errors(vlscan_ctx* ctx) {
     unsigned long long h[ST_COUNT];
     VL_CUDA(cudaMemcpyAsync(h, ctx->gstat.p, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1345,6 +1349,19 @@ static void check_gather_errors(vlscan_ctx* ctx) {
                                       "the decoded timestamps of a block contradict the minimum / maximum of its header"};
     if (h[ST_ERROR]) throw BadInput(msg[std::min<unsigned long long>(h[ST_ERROR], 9)]);
 }
+// the timestamps of the blocks in `list` (wc[WC_ROW] of them) decoded into ctx->ts_vals, at each block's first word * 64; errors go to gstat
+static const unsigned long long* decode_listed_timestamps(vlscan_ctx* ctx, const BatchView& B, const uint32_t* list, const uint32_t* wc) {
+    ctx->ts_vals.ensure(B.nwords * 64 * 8);
+    k_ts_decode_list<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(B, list, wc, ctx->ts_vals.as<unsigned long long>(), ctx->gstat.as<unsigned long long>()); launch_check(ctx);
+    return ctx->ts_vals.as<unsigned long long>();
+}
+// the canonical names of a caller's n field names ("" is `_msg`: getCanonicalColumnName)
+static std::vector<std::string> canonical_names(const char* const* names, const size_t* lens, uint32_t n, const char* what) {
+    if (n && (!names || !lens)) throw BadInput(std::string(what) + ": field names missing");
+    std::vector<std::string> out;
+    for (uint32_t f = 0; f < n; f++) out.push_back(lens[f] ? std::string(names[f], lens[f]) : "_msg");
+    return out;
+}
 
 int vlscan_gather_timestamps(vlscan_ctx* ctx, int64_t* out_timestamps, uint64_t cap, uint64_t* out_hit_offsets) {
     return guarded(ctx, [&] {
@@ -1354,13 +1371,11 @@ int vlscan_gather_timestamps(vlscan_ctx* ctx, int64_t* out_timestamps, uint64_t 
         const vlscan_batch* b = ctx->last_batch;
         BatchView B = b->view();
         uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* row_blocks = ctx->row_blocks.as<uint32_t>();
-        unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
         VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
         k_hit_blocks_list<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), -1, 1, row_blocks, wc); launch_check(ctx);
-        ctx->ts_vals.ensure(b->nwords * 64 * 8);
-        k_ts_decode_list<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(B, row_blocks, wc, ctx->ts_vals.as<unsigned long long>(), gstat); launch_check(ctx);
+        const unsigned long long* ts_vals = decode_listed_timestamps(ctx, B, row_blocks, wc);
         ctx->gout.ensure(n * 8);
-        k_gather_ts<<<cdiv(n, 256), 256, 0, ctx->stream>>>(B, ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), n, ctx->ts_vals.as<unsigned long long>(), ctx->gout.as<long long>()); launch_check(ctx);
+        k_gather_ts<<<cdiv(n, 256), 256, 0, ctx->stream>>>(B, ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), n, ts_vals, ctx->gout.as<long long>()); launch_check(ctx);
         check_gather_errors(ctx);
         VL_CUDA(cudaMemcpy(out_timestamps, ctx->gout.p, n * 8, cudaMemcpyDeviceToHost));
     });
@@ -1395,16 +1410,21 @@ static const uint32_t* hit_row_offsets(vlscan_ctx* ctx, int slot, const std::str
     k_lens_offsets<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(B, slot, ctx->lens_blocks.as<uint32_t>(), wc, ctx->row_off8[slot].as<uint32_t>(), ready, ctx->gstat.as<unsigned long long>()); launch_check(ctx);
     return ctx->row_off8[slot].as<uint32_t>();
 }
+// exclusive scan of the n lengths into offs[0 .. n], offs[n] = the total: tile sums, their scan by one CTA, per-tile prefixes
+static void exclusive_scan(vlscan_ctx* ctx, const uint32_t* lens, uint64_t n, uint64_t* offs) {
+    const uint64_t ntiles = cdiv(n, VL_SCAN_TILE);
+    ctx->gtiles.ensure((ntiles + 1) * 8);
+    k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(lens, n, ctx->gtiles.as<unsigned long long>(), nullptr, 0); launch_check(ctx);
+    k_scan_cta<uint64_t><<<1, 1024, 0, ctx->stream>>>(ctx->gtiles.as<uint64_t>(), (uint32_t)ntiles, ctx->gtiles.as<uint64_t>(), offs + n); launch_check(ctx);
+    k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(lens, n, ctx->gtiles.as<unsigned long long>(), (unsigned long long*)offs, 1); launch_check(ctx);
+}
 // texts of column `slot` in the n rows (rows[i], blocks[i]): their lengths and exclusive offsets go to ctx->glens / ctx->goffs (goffs[n] = the
 // total, also returned; synchronises), then text_bytes writes the bytes to ctx->gout
 static uint64_t text_offsets(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint32_t* rows, const uint32_t* blocks, uint64_t n) {
     BatchView B = ctx->last_batch->view();
-    const uint64_t ntiles = cdiv(n, VL_SCAN_TILE);
-    ctx->glens.ensure(n * 4); ctx->goffs.ensure((n + 1) * 8); ctx->gtiles.ensure((ntiles + 1) * 8);
+    ctx->glens.ensure(n * 4); ctx->goffs.ensure((n + 1) * 8);
     k_gather_values<<<cdiv(n, 128), 128, 0, ctx->stream>>>(B, slot, rows, blocks, n, ro, 0, ctx->glens.as<uint32_t>(), nullptr, nullptr, ctx->gstat.as<unsigned long long>()); launch_check(ctx);
-    k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(ctx->glens.as<uint32_t>(), n, ctx->gtiles.as<unsigned long long>(), nullptr, 0); launch_check(ctx);
-    k_scan_tile_sums<<<1, 1024, 0, ctx->stream>>>(ctx->gtiles.as<unsigned long long>(), ntiles, ctx->goffs.as<unsigned long long>() + n); launch_check(ctx);
-    k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(ctx->glens.as<uint32_t>(), n, ctx->gtiles.as<unsigned long long>(), ctx->goffs.as<unsigned long long>(), 1); launch_check(ctx);
+    exclusive_scan(ctx, ctx->glens.as<uint32_t>(), n, ctx->goffs.as<uint64_t>());
     uint64_t total = 0;
     VL_CUDA(cudaMemcpyAsync(&total, ctx->goffs.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
     check_gather_errors(ctx);
@@ -1414,6 +1434,29 @@ static void text_bytes(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint
     ctx->gout.ensure(std::max<uint64_t>(total, 16));
     k_gather_values<<<cdiv(n, 128), 128, 0, ctx->stream>>>(ctx->last_batch->view(), slot, rows, blocks, n, ro, 1, nullptr, ctx->goffs.as<uint64_t>(), ctx->gout.as<uint8_t>(), ctx->gstat.as<unsigned long long>());
     launch_check(ctx);
+}
+// the texts of column `slot` in the n rows (rows[i], blocks[i]) on the host: text i is bytes[offs[i] .. offs[i + 1])
+static void host_texts(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint32_t* rows, const uint32_t* blocks, uint64_t n, std::vector<uint64_t>& offs,
+                       std::vector<uint8_t>& bytes) {
+    const uint64_t total = text_offsets(ctx, slot, ro, rows, blocks, n);
+    offs.resize(n + 1); bytes.resize(total);
+    text_bytes(ctx, slot, ro, rows, blocks, n, total);
+    VL_CUDA(cudaMemcpyAsync(offs.data(), ctx->goffs.p, (n + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (total) VL_CUDA(cudaMemcpyAsync(bytes.data(), ctx->gout.p, total, cudaMemcpyDeviceToHost, ctx->stream));
+    check_gather_errors(ctx);   // synchronises
+}
+// rows x fields output: row i is row order[i] of the per-field texts (host_texts); the text of field f in row i ends at out_offsets[i * nf + f + 1]
+static void pack_texts(const std::vector<uint64_t>& order, const std::vector<std::vector<uint64_t>>& toffs, const std::vector<std::vector<uint8_t>>& tbytes,
+                       uint8_t* out_bytes, uint64_t* out_offsets) {
+    const size_t nf = toffs.size();
+    uint64_t o = 0;
+    for (uint64_t i = 0; i < order.size(); i++)
+        for (size_t f = 0; f < nf; f++) {
+            const uint64_t a = toffs[f][order[i]], len = toffs[f][order[i] + 1] - a;
+            if (len) memcpy(out_bytes + o, tbytes[f].data() + a, len);
+            o += len;
+            out_offsets[i * nf + f + 1] = o;
+        }
 }
 
 int vlscan_gather_values(vlscan_ctx* ctx, const char* field, size_t field_len, uint8_t* out_bytes, uint64_t cap_bytes, uint64_t* out_value_offsets, uint64_t cap_values,
@@ -1448,13 +1491,9 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
         if (!q) throw BadInput("no hits query");
         if (q->calendar > VLSCAN_BUCKET_YEAR) throw BadInput("unknown calendar bucket kind");
         if (q->nby > VLSCAN_HITS_MAX_BY) throw BadInput("too many by-fields for the hits aggregation (at most VLSCAN_HITS_MAX_BY = 4)");
-        std::vector<std::string> names;
-        for (uint32_t f = 0; f < q->nby; f++) {
-            std::string n(q->by_names[f], q->by_name_lens[f]);
-            if (n.empty()) n = "_msg";   // getCanonicalColumnName
+        const std::vector<std::string> names = canonical_names(q->by_names, q->by_name_lens, q->nby, "vlscan_hits_stats");
+        for (const std::string& n : names)
             if (n == "_time") throw BadInput("`_time` cannot be a by-field of the hits aggregation: it is the bucket");
-            names.push_back(n);
-        }
         if (!ctx) throw BadInput("vlscan_hits_stats needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
         const uint64_t n = build_hit_list(ctx, nullptr);
         if (n >= 0xFFFFFFFFull) throw BadInput("more than 2^32 - 2 selected rows in one batch");
@@ -1470,25 +1509,23 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
         // buckets of the blocks; timestamps decoded only where a block spans several buckets
         unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
         uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* row_blocks = ctx->row_blocks.as<uint32_t>();
-        ctx->hblk.ensure(b->nblocks * 9 + 16);
-        long long* blk_bucket = ctx->hblk.as<long long>(); uint8_t* blk_multi = ctx->hblk.as<uint8_t>() + b->nblocks * 8;
+        long long* blk_bucket; uint8_t* blk_multi;
+        Carve().take(blk_bucket, b->nblocks).take(blk_multi, b->nblocks).place(ctx->hblk);
         VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
         k_hits_classify<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), hq, blk_bucket, blk_multi, row_blocks, wc, gstat); launch_check(ctx);
-        ctx->ts_vals.ensure(b->nwords * 64 * 8);
-        k_ts_decode_list<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(B, row_blocks, wc, ctx->ts_vals.as<unsigned long long>(), gstat); launch_check(ctx);
+        const unsigned long long* ts_vals = decode_listed_timestamps(ctx, B, row_blocks, wc);
         uint32_t decoded = 0;
         VL_CUDA(cudaMemcpyAsync(&decoded, wc + WC_ROW, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        HitsView V{ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), blk_bucket, blk_multi, ctx->ts_vals.as<unsigned long long>()};
+        HitsView V{ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), blk_bucket, blk_multi, ts_vals};
         // the group table: starts small, grows by 8x while a pass overflows; at 2 x the hit count it cannot overflow
         uint64_t max_cap = 1024; while (max_cap < 2 * n) max_cap <<= 1;
         uint64_t cap = std::min<uint64_t>(max_cap, 1 << 14);
         HitsTable T;
         unsigned long long state[3];
         for (;;) {
-            ctx->htab.ensure(cap * 16 + 32);
-            T.tags = ctx->htab.as<unsigned long long>(); T.cnt = T.tags + cap; T.state = T.cnt + cap;
+            const size_t bytes = Carve().take(T.tags, cap).take(T.cnt, cap).take(T.state, 4).place(ctx->htab);
             T.mask = cap - 1; T.limit = cap == max_cap ? cap : cap / 2;
-            VL_CUDA(cudaMemsetAsync(T.tags, 0, cap * 16 + 32, ctx->stream));
+            VL_CUDA(cudaMemsetAsync(T.tags, 0, bytes, ctx->stream));
             k_hits_group<<<(unsigned)std::min<uint64_t>(b->nblocks, (uint64_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(B, hq, V, T, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat);
             launch_check(ctx);
             VL_CUDA(cudaMemcpyAsync(state, T.state, sizeof state, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1501,9 +1538,8 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
         const uint64_t G = state[0];
         info[0] = G; info[3] = decoded;
         // the groups, then the texts of their representatives only
-        ctx->hgrp.ensure(G * 24 + 64);
-        long long* buckets = ctx->hgrp.as<long long>(); unsigned long long* counts = (unsigned long long*)(buckets + G);
-        uint32_t* rep_rows = (uint32_t*)(counts + G); uint32_t* rep_blocks = rep_rows + G;
+        long long* buckets; unsigned long long* counts; uint32_t* rep_rows; uint32_t* rep_blocks;
+        Carve().take(buckets, G).take(counts, G).take(rep_rows, G).take(rep_blocks, G).place(ctx->hgrp);
         k_hits_emit<<<cdiv(cap, 256), 256, 0, ctx->stream>>>(B, hq, V, T, rep_rows, rep_blocks, buckets, counts); launch_check(ctx);
         std::vector<int64_t> hb(G); std::vector<uint64_t> hc(G);
         VL_CUDA(cudaMemcpyAsync(hb.data(), buckets, G * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1511,13 +1547,8 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
         std::vector<std::vector<uint64_t>> toffs(q->nby); std::vector<std::vector<uint8_t>> tbytes(q->nby);
         uint64_t key_bytes = 0;
         for (uint32_t f = 0; f < q->nby; f++) {
-            const uint64_t total = text_offsets(ctx, hq.slot[f], hq.row_off8[f], rep_rows, rep_blocks, G);
-            key_bytes += total;
-            toffs[f].resize(G + 1); tbytes[f].resize(total);
-            text_bytes(ctx, hq.slot[f], hq.row_off8[f], rep_rows, rep_blocks, G, total);
-            VL_CUDA(cudaMemcpyAsync(toffs[f].data(), ctx->goffs.p, (G + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
-            if (total) VL_CUDA(cudaMemcpyAsync(tbytes[f].data(), ctx->gout.p, total, cudaMemcpyDeviceToHost, ctx->stream));
-            VL_CUDA(cudaStreamSynchronize(ctx->stream));
+            host_texts(ctx, hq.slot[f], hq.row_off8[f], rep_rows, rep_blocks, G, toffs[f], tbytes[f]);
+            key_bytes += tbytes[f].size();
         }
         VL_CUDA(cudaStreamSynchronize(ctx->stream));
         info[1] = key_bytes;
@@ -1533,16 +1564,8 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
             for (uint32_t f = 0; f < q->nby; f++) { const int c = text(f, x).compare(text(f, y)); if (c) return c < 0; }
             return false;
         });
-        uint64_t o = 0;
-        for (uint64_t i = 0; i < G; i++) {
-            const uint64_t g = order[i];
-            out_buckets[i] = hb[g]; out_counts[i] = hc[g];
-            for (uint32_t f = 0; f < q->nby; f++) {
-                const std::string_view t = text(f, g);
-                memcpy(out_key_bytes + o, t.data(), t.size()); o += t.size();
-                out_key_offsets[i * q->nby + f + 1] = o;
-            }
-        }
+        for (uint64_t i = 0; i < G; i++) { out_buckets[i] = hb[order[i]]; out_counts[i] = hc[order[i]]; }
+        pack_texts(order, toffs, tbytes, out_key_bytes, out_key_offsets);
     });
     if (out_info) memcpy(out_info, info, sizeof info);
     return rc;
@@ -1567,14 +1590,9 @@ int vlscan_last_rows(vlscan_ctx* ctx, const vlscan_last_query* q, int64_t* out_t
     const int rc = guarded(ctx, [&] {
         if (!q) throw BadInput("no last-rows query");
         if (q->limit == 0) throw BadInput("the limit of vlscan_last_rows must be at least 1");
-        if (q->nfields && (!q->field_names || !q->field_name_lens)) throw BadInput("vlscan_last_rows: field names missing");
-        std::vector<std::string> names;
-        for (uint32_t f = 0; f < q->nfields; f++) {
-            std::string n(q->field_names[f], q->field_name_lens[f]);
-            if (n.empty()) n = "_msg";   // getCanonicalColumnName
+        const std::vector<std::string> names = canonical_names(q->field_names, q->field_name_lens, q->nfields, "vlscan_last_rows");
+        for (const std::string& n : names)
             if (n == "_time") throw BadInput("`_time` cannot be a field of vlscan_last_rows: it is returned in out_timestamps");
-            names.push_back(n);
-        }
         if (!ctx) throw BadInput("vlscan_last_rows needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
         if (!ctx->has_result) throw BadInput("no scan result on this ctx");
         VL_CUDA(cudaSetDevice(ctx->device));
@@ -1586,32 +1604,30 @@ int vlscan_last_rows(vlscan_ctx* ctx, const vlscan_last_query* q, int64_t* out_t
         ctx->gstat.ensure(ST_COUNT * 8);
         VL_CUDA(cudaMemsetAsync(ctx->gstat.p, 0, ST_COUNT * 8, ctx->stream));
         unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
-        ctx->hblk.ensure(nb * 28 + 64);
-        long long* blk_key = ctx->hblk.as<long long>();
-        uint64_t* cand_offs = (uint64_t*)(blk_key + nb);
-        uint32_t* blk_w = (uint32_t*)(cand_offs + nb + 1); uint32_t* cand_rows = blk_w + nb; uint32_t* blk_mark = cand_rows + nb;
+        long long* blk_key; uint64_t* cand_offs; uint32_t* blk_w; uint32_t* cand_rows; uint32_t* blk_mark; uint32_t* cand; uint32_t* decode;
+        Carve().take(blk_key, nb).take(cand_offs, nb + 1).take(blk_w, nb).take(cand_rows, nb).take(blk_mark, nb).take(cand, nb).take(decode, nb).place(ctx->hblk);
         const size_t st_words = RS_COUNT + VL_RADIX_PASSES * 256;
-        ctx->htab.ensure(2 * st_words * 8);
-        unsigned long long* st_blk = ctx->htab.as<unsigned long long>(); unsigned long long* st_row = st_blk + st_words;
-        ctx->hit_offs.ensure((nb + 1) * 8); ctx->lens_blocks2.ensure(nb * 4 + 16); ctx->row_blocks.ensure(nb * 4 + 16);
-        k_scan_counts<<<1, 1024, 0, ctx->stream>>>(counts, (uint32_t)nb, ctx->hit_offs.as<uint64_t>()); launch_check(ctx);
+        unsigned long long* st_blk; unsigned long long* st_row;
+        Carve().take(st_blk, st_words).take(st_row, st_words).place(ctx->htab);
+        ctx->hit_offs.ensure((nb + 1) * 8);
+        uint64_t* hit_offs = ctx->hit_offs.as<uint64_t>();
+        k_scan_cta<uint32_t><<<1, 1024, 0, ctx->stream>>>(counts, (uint32_t)nb, hit_offs, hit_offs + nb); launch_check(ctx);
         // (1) the block threshold T_lo, from the headers alone
         if (nb) { k_last_block_keys<<<cdiv(nb, 256), 256, 0, ctx->stream>>>(B, counts, floor_ts, blk_key, blk_w, gstat); launch_check(ctx); }
         radix_select(ctx, blk_key, blk_w, nb, limit, st_blk);
         // (2) the candidate blocks, the timestamps of those that are not flat, and the count of their selected rows >= T_lo
-        uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* cand = ctx->lens_blocks2.as<uint32_t>(); uint32_t* decode = ctx->row_blocks.as<uint32_t>();
+        uint32_t* wc = ctx->work_count.as<uint32_t>();
         VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
-        VL_CUDA(cudaMemsetAsync(cand_rows, 0, nb * 8, ctx->stream));   // cand_rows and blk_mark
+        VL_CUDA(cudaMemsetAsync(cand_rows, 0, nb * 4, ctx->stream));
+        VL_CUDA(cudaMemsetAsync(blk_mark, 0, nb * 4, ctx->stream));
         if (nb) { k_last_candidates<<<cdiv(nb, 256), 256, 0, ctx->stream>>>(B, counts, floor_ts, st_blk, cand, decode, wc); launch_check(ctx); }
-        ctx->ts_vals.ensure(b->nwords * 64 * 8);
-        unsigned long long* ts_vals = ctx->ts_vals.as<unsigned long long>();
-        k_ts_decode_list<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(B, decode, wc, ts_vals, gstat); launch_check(ctx);
+        const unsigned long long* ts_vals = decode_listed_timestamps(ctx, B, decode, wc);
         const unsigned row_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(nb, (uint64_t)ctx->sm_count * 8));
         k_last_rows<<<row_grid, 256, 0, ctx->stream>>>(B, ctx->regs[0].as<uint64_t>(), cand, wc, ts_vals, floor_ts, st_blk, 0, cand_rows, nullptr, nullptr, nullptr, nullptr, gstat);
         launch_check(ctx);
-        k_scan_counts<<<1, 1024, 0, ctx->stream>>>(cand_rows, (uint32_t)nb, cand_offs); launch_check(ctx);
+        k_scan_cta<uint32_t><<<1, 1024, 0, ctx->stream>>>(cand_rows, (uint32_t)nb, cand_offs, cand_offs + nb); launch_check(ctx);
         uint64_t selected = 0, M = 0; unsigned long long blk_short = 0; uint32_t decoded = 0;
-        VL_CUDA(cudaMemcpyAsync(&selected, ctx->hit_offs.as<uint64_t>() + nb, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaMemcpyAsync(&selected, hit_offs + nb, 8, cudaMemcpyDeviceToHost, ctx->stream));
         VL_CUDA(cudaMemcpyAsync(&M, cand_offs + nb, 8, cudaMemcpyDeviceToHost, ctx->stream));
         VL_CUDA(cudaMemcpyAsync(&blk_short, st_blk + RS_SHORT, 8, cudaMemcpyDeviceToHost, ctx->stream));
         VL_CUDA(cudaMemcpyAsync(&decoded, wc + WC_ROW, 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1625,20 +1641,16 @@ int vlscan_last_rows(vlscan_ctx* ctx, const vlscan_last_query* q, int64_t* out_t
         uint32_t* sel_blk = nullptr; uint32_t* sel_row = nullptr;
         if (n) {
             // the candidates in (block, row) order, then (3) the exact top N: T_N, every row above it and the last ties
-            ctx->lcand.ensure(M * 16 + 64);
-            long long* cts = ctx->lcand.as<long long>(); uint32_t* cblk = (uint32_t*)(cts + M); uint32_t* crow = cblk + M;
+            long long* cts; uint32_t* cblk; uint32_t* crow;
+            Carve().take(cts, M).take(cblk, M).take(crow, M).place(ctx->lcand);
             k_last_rows<<<row_grid, 256, 0, ctx->stream>>>(B, ctx->regs[0].as<uint64_t>(), cand, wc, ts_vals, floor_ts, st_blk, 1, nullptr, cand_offs, cts, cblk, crow, gstat);
             launch_check(ctx);
             radix_select(ctx, cts, nullptr, M, limit, st_row);
-            const uint64_t ntiles = cdiv(M, VL_SCAN_TILE);
-            ctx->glens.ensure(M * 4); ctx->goffs.ensure((M + 1) * 8); ctx->gtiles.ensure((ntiles + 1) * 8);
+            ctx->glens.ensure(M * 4); ctx->goffs.ensure((M + 1) * 8);
             k_last_ties<<<cdiv(M, 256), 256, 0, ctx->stream>>>(cts, M, st_row, ctx->glens.as<uint32_t>()); launch_check(ctx);
-            k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(ctx->glens.as<uint32_t>(), M, ctx->gtiles.as<unsigned long long>(), nullptr, 0); launch_check(ctx);
-            k_scan_tile_sums<<<1, 1024, 0, ctx->stream>>>(ctx->gtiles.as<unsigned long long>(), ntiles, ctx->goffs.as<unsigned long long>() + M); launch_check(ctx);
-            k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(ctx->glens.as<uint32_t>(), M, ctx->gtiles.as<unsigned long long>(), ctx->goffs.as<unsigned long long>(), 1); launch_check(ctx);
-            ctx->hgrp.ensure(n * 16 + 64);
-            long long* sel_ts = ctx->hgrp.as<long long>(); unsigned long long* sel_n = (unsigned long long*)(sel_ts + n);
-            sel_blk = (uint32_t*)(sel_n + 1); sel_row = sel_blk + n;
+            exclusive_scan(ctx, ctx->glens.as<uint32_t>(), M, ctx->goffs.as<uint64_t>());
+            long long* sel_ts; unsigned long long* sel_n;
+            Carve().take(sel_ts, n).take(sel_n, 1).take(sel_blk, n).take(sel_row, n).place(ctx->hgrp);
             VL_CUDA(cudaMemsetAsync(sel_n, 0, 8, ctx->stream));
             k_last_choose<<<cdiv(M, 256), 256, 0, ctx->stream>>>(cts, cblk, crow, M, st_row, ctx->goffs.as<uint64_t>(), sel_ts, sel_blk, sel_row, sel_n, blk_mark); launch_check(ctx);
             uint64_t chosen = 0;
@@ -1654,16 +1666,10 @@ int vlscan_last_rows(vlscan_ctx* ctx, const vlscan_last_query* q, int64_t* out_t
         uint64_t value_bytes = 0;
         for (uint32_t f = 0; f < q->nfields && n; f++) {
             const int slot = field_slot(b, names[f]);
-            const uint32_t* ro = hit_row_offsets(ctx, slot, names[f], blk_mark);
-            const uint64_t total = text_offsets(ctx, slot, ro, sel_row, sel_blk, n);
-            value_bytes += total;
-            toffs[f].resize(n + 1); tbytes[f].resize(total);
-            text_bytes(ctx, slot, ro, sel_row, sel_blk, n, total);
-            VL_CUDA(cudaMemcpyAsync(toffs[f].data(), ctx->goffs.p, (n + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
-            if (total) VL_CUDA(cudaMemcpyAsync(tbytes[f].data(), ctx->gout.p, total, cudaMemcpyDeviceToHost, ctx->stream));
-            VL_CUDA(cudaStreamSynchronize(ctx->stream));
+            host_texts(ctx, slot, hit_row_offsets(ctx, slot, names[f], blk_mark), sel_row, sel_blk, n, toffs[f], tbytes[f]);
+            value_bytes += tbytes[f].size();
         }
-        check_gather_errors(ctx);
+        if (!q->nfields) check_gather_errors(ctx);   // else host_texts checked them after the last kernel
         info[0] = n; info[1] = value_bytes;
         if (n > cap_rows) throw BadInput("rows buffer too small (the needed size is reported)");
         if (value_bytes > cap_bytes) throw BadInput("value bytes buffer too small (the needed size is reported)");
@@ -1677,17 +1683,8 @@ int vlscan_last_rows(vlscan_ctx* ctx, const vlscan_last_query* q, int64_t* out_t
             return hr[x] < hr[y];
         });
         if (out_offsets) out_offsets[0] = 0;
-        uint64_t o = 0;
-        for (uint64_t i = 0; i < n; i++) {
-            const uint64_t k = order[i];
-            out_timestamps[i] = hts[k]; out_blocks[i] = hb[k]; out_rows[i] = hr[k];
-            for (uint32_t f = 0; f < q->nfields; f++) {
-                const uint64_t a = toffs[f][k], len = toffs[f][k + 1] - a;
-                if (len) memcpy(out_bytes + o, tbytes[f].data() + a, len);
-                o += len;
-                out_offsets[i * q->nfields + f + 1] = o;
-            }
-        }
+        for (uint64_t i = 0; i < n; i++) { out_timestamps[i] = hts[order[i]]; out_blocks[i] = hb[order[i]]; out_rows[i] = hr[order[i]]; }
+        pack_texts(order, toffs, tbytes, out_bytes, out_offsets);
     });
     if (out_info) memcpy(out_info, info, sizeof info);
     return rc;
@@ -1716,14 +1713,10 @@ int vlscan_facets(vlscan_ctx* ctx, const vlscan_facets_query* q, uint8_t* out_dr
     const int rc = guarded(ctx, [&] {
         if (!q) throw BadInput("no facets query");
         if (q->nfields == 0) throw BadInput("vlscan_facets needs at least one field");
-        if (!q->field_names || !q->field_name_lens) throw BadInput("vlscan_facets: field names missing");
-        std::vector<std::string> names;
-        for (uint32_t f = 0; f < q->nfields; f++) {
-            std::string n(q->field_names[f], q->field_name_lens[f]);
-            if (n.empty()) n = "_msg";   // getCanonicalColumnName
-            if (n == "_stream" || n == "_stream_id") throw BadInput("`" + n + "` facets are not computed by the engine: it does not know the streams of the blocks");
-            if (std::find(names.begin(), names.end(), n) != names.end()) throw BadInput("duplicate facets field `" + n + "`");
-            names.push_back(n);
+        const std::vector<std::string> names = canonical_names(q->field_names, q->field_name_lens, q->nfields, "vlscan_facets");
+        for (auto n = names.begin(); n != names.end(); ++n) {
+            if (*n == "_stream" || *n == "_stream_id") throw BadInput("`" + *n + "` facets are not computed by the engine: it does not know the streams of the blocks");
+            if (std::find(names.begin(), n, *n) != n) throw BadInput("duplicate facets field `" + *n + "`");
         }
         const uint64_t max_values = q->max_values_per_field ? q->max_values_per_field : VLSCAN_FACETS_DEFAULT_MAX_VALUES;
         const uint64_t max_len = q->max_value_len ? q->max_value_len : VLSCAN_FACETS_DEFAULT_MAX_VALUE_LEN;
@@ -1741,15 +1734,8 @@ int vlscan_facets(vlscan_ctx* ctx, const vlscan_facets_query* q, uint8_t* out_dr
             const vlscan_batch* b = ctx->last_batch;
             BatchView B = b->view();
             // small device state: the field table, the entry bases and cursors, a work counter, a flag, the blocks with hits
-            size_t off = 0;
-            auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 15) & ~(size_t)15; return o; };
-            const size_t o_fields = take(nf * sizeof(FacetField)), o_base = take((nf + 1) * 8), o_cursor = take(nf * 8), o_wc = take(WC_COUNT * 4), o_flag = take(4),
-                         o_blocks = take(b->nblocks * 4 + 4);
-            ctx->hblk.ensure(off);
-            uint8_t* hb = ctx->hblk.as<uint8_t>();
-            FacetField* d_fields = (FacetField*)(hb + o_fields);
-            uint64_t* d_base = (uint64_t*)(hb + o_base); unsigned long long* d_cursor = (unsigned long long*)(hb + o_cursor);
-            uint32_t* d_wc = (uint32_t*)(hb + o_wc); unsigned int* d_flag = (unsigned int*)(hb + o_flag); uint32_t* d_blocks = (uint32_t*)(hb + o_blocks);
+            FacetField* d_fields; uint64_t* d_base; unsigned long long* d_cursor; uint32_t* d_wc; unsigned int* d_flag; uint32_t* d_blocks;
+            Carve().take(d_fields, nf).take(d_base, nf + 1).take(d_cursor, nf).take(d_wc, WC_COUNT).take(d_flag, 1).take(d_blocks, b->nblocks + 1).place(ctx->hblk);
             VL_CUDA(cudaMemsetAsync(d_wc, 0, WC_COUNT * 4, ctx->stream));
             k_hit_blocks_list<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), -1, 1, d_blocks, d_wc); launch_check(ctx);
             uint32_t nblk = 0;
@@ -1807,10 +1793,8 @@ int vlscan_facets(vlscan_ctx* ctx, const vlscan_facets_query* q, uint8_t* out_dr
                 uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* row_blocks = ctx->row_blocks.as<uint32_t>();
                 VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
                 k_facets_ts_list<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, A.counts, row_blocks, wc, gstat); launch_check(ctx);
-                ctx->ts_vals.ensure(b->nwords * 64 * 8);
-                k_ts_decode_list<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(B, row_blocks, wc, ctx->ts_vals.as<unsigned long long>(), gstat); launch_check(ctx);
+                A.ts_vals = decode_listed_timestamps(ctx, B, row_blocks, wc);
                 VL_CUDA(cudaMemcpyAsync(&decoded, wc + WC_ROW, 4, cudaMemcpyDeviceToHost, ctx->stream));
-                A.ts_vals = ctx->ts_vals.as<unsigned long long>();
                 check_gather_errors(ctx);
             }
             info[3] = decoded;
@@ -1825,10 +1809,8 @@ int vlscan_facets(vlscan_ctx* ctx, const vlscan_facets_query* q, uint8_t* out_dr
             }
             const uint64_t E = field_off[nf];
             std::vector<uint32_t> cls(E), rrows(E), rblocks(E); std::vector<unsigned long long> nums(E), cnts(E);
-            ctx->hgrp.ensure(E * 40 + 64);
-            uint32_t* rep_rows = ctx->hgrp.as<uint32_t>(); uint32_t* rep_blocks = rep_rows + E; uint32_t* d_cls = rep_blocks + E;
-            unsigned long long* d_nums = (unsigned long long*)(ctx->hgrp.as<uint8_t>() + ((E * 12 + 7) & ~7ull)); unsigned long long* d_cnts = d_nums + E;
-            uint32_t* str_rows = (uint32_t*)(d_cnts + E); uint32_t* str_blocks = str_rows + E;
+            uint32_t* rep_rows; uint32_t* rep_blocks; uint32_t* d_cls; unsigned long long* d_nums; unsigned long long* d_cnts; uint32_t* str_rows; uint32_t* str_blocks;
+            Carve().take(rep_rows, E).take(rep_blocks, E).take(d_cls, E).take(d_nums, E).take(d_cnts, E).take(str_rows, E).take(str_blocks, E).place(ctx->hgrp);
             if (E) {   // the entries field after field
                 VL_CUDA(cudaMemcpyAsync(d_base, field_off.data(), nf * 8, cudaMemcpyHostToDevice, ctx->stream));
                 VL_CUDA(cudaMemsetAsync(d_cursor, 0, nf * 8, ctx->stream));
@@ -1848,18 +1830,13 @@ int vlscan_facets(vlscan_ctx* ctx, const vlscan_facets_query* q, uint8_t* out_dr
                 std::vector<uint64_t> str_of; std::vector<uint32_t> sr, sb;
                 for (uint64_t i = 0; i < ne; i++)
                     if (cls[e0 + i] == FK_STR) { str_of.push_back(i); sr.push_back(rrows[e0 + i]); sb.push_back(rblocks[e0 + i]); }
-                std::vector<uint64_t> toffs; std::string tbytes;
                 if (!str_of.empty()) {
                     const uint64_t ns = str_of.size();
                     VL_CUDA(cudaMemcpyAsync(str_rows, sr.data(), ns * 4, cudaMemcpyHostToDevice, ctx->stream));
                     VL_CUDA(cudaMemcpyAsync(str_blocks, sb.data(), ns * 4, cudaMemcpyHostToDevice, ctx->stream));
-                    const uint64_t total = text_offsets(ctx, hf[f].slot, hf[f].row_off8, str_rows, str_blocks, ns);
-                    toffs.resize(ns + 1); tbytes.resize(total);
-                    text_bytes(ctx, hf[f].slot, hf[f].row_off8, str_rows, str_blocks, ns, total);
-                    VL_CUDA(cudaMemcpyAsync(toffs.data(), ctx->goffs.p, (ns + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
-                    if (total) VL_CUDA(cudaMemcpyAsync(&tbytes[0], ctx->gout.p, total, cudaMemcpyDeviceToHost, ctx->stream));
-                    check_gather_errors(ctx);
-                    for (uint64_t k = 0; k < ns; k++) text[str_of[k]] = tbytes.substr(toffs[k], toffs[k + 1] - toffs[k]);
+                    std::vector<uint64_t> toffs; std::vector<uint8_t> tbytes;
+                    host_texts(ctx, hf[f].slot, hf[f].row_off8, str_rows, str_blocks, ns, toffs, tbytes);
+                    for (uint64_t k = 0; k < ns; k++) text[str_of[k]].assign((const char*)tbytes.data() + toffs[k], toffs[k + 1] - toffs[k]);
                 }
                 std::vector<uint8_t> ecl(ne);
                 for (uint64_t i = 0; i < ne; i++) {
@@ -2051,7 +2028,7 @@ int vlscan_stage_selected(vlscan_ctx* ctx, const vlscan_block* blocks, uint64_t 
     bool staging = false;
     const int rc = guarded(ctx, [&] {
         if (nfields == 0) throw BadInput("vlscan_stage_selected needs at least one field");
-        if (!field_names || !field_name_lens) throw BadInput("vlscan_stage_selected: field names missing");
+        const std::vector<std::string> names = canonical_names(field_names, field_name_lens, nfields, "vlscan_stage_selected");
         if (nlist && !block_list) throw BadInput("vlscan_stage_selected: block list missing");
         if (!ctx) throw BadInput("vlscan_stage_selected needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
         if (!ctx->has_result || !ctx->kept || !ctx->recycle || ctx->last_batch != ctx->recycle) throw BadInput("no kept scan on this ctx (vlscan_scan_batch_keep keeps one until the next scan)");
@@ -2059,9 +2036,7 @@ int vlscan_stage_selected(vlscan_ctx* ctx, const vlscan_block* blocks, uint64_t 
         VL_CUDA(cudaSetDevice(ctx->device));
         const uint32_t nf = b->nfields;
         std::vector<char> want(nf, 0);
-        for (uint32_t f = 0; f < nfields; f++) {
-            std::string n(field_names[f], field_name_lens[f]);
-            if (n.empty()) n = "_msg";   // getCanonicalColumnName
+        for (const std::string& n : names) {
             const int slot = field_slot(b, n);
             if (slot < 0) throw BadInput("field `" + n + "` is not a field of the kept batch");
             want[slot] = 1;

@@ -99,16 +99,25 @@ struct vlscan_ctx {
     std::string err;
     uint64_t launches = 0;
     // scratch (grow-only)
-    vl::DevBuf action, payload, leaf_bm, lens_blocks, row_blocks, work_count, stats, totals, counts, slots, hit_offs, hits, lens_blocks2, tiles;   // lens_blocks2: second lens work list of a two-column leaf; tiles: ScanTile work list of k_substr_scan
+    vl::DevBuf action, payload, leaf_bm, lens_blocks, work_count, stats, totals, counts, slots, tiles;   // tiles: ScanTile work list of k_substr_scan
+    vl::DevBuf lens_blocks2;               // second lens work list of a two-column leaf
+    vl::DevBuf row_blocks;                 // block work list: row-level blocks of the scan; the timestamps decode list of vlscan_gather_timestamps,
+                                           // vlscan_hits_stats and vlscan_facets
+    vl::DevBuf hit_offs, hits;             // build_hit_list: first hit of every block, row of each hit (hit_offs also: vlscan_last_rows' selected
+                                           // row count, vlscan_result_digest's digest)
     std::vector<vl::DevBuf> regs;          // bitmap registers of the tree interpreter
     std::vector<vl::DevBuf> row_off8;      // per batch field slot: byte offset of every 8th row (k_lens_offsets)
     std::vector<vl::DevBuf> ready;         // per batch field slot: row_off8 computed for block b in this scan
     std::vector<char> ready_cleared;
-    vl::DevBuf hit_block, glens, goffs, gtiles, gout, gstat;   // hit materialisation (vlscan_gather_*): block of each hit, value lengths / offsets, output staging, error slot
-    vl::DevBuf ts_vals;                    // decoded timestamps / running sums, 8 bytes per row of the batch (k_time_match, gather)
-    vl::DevBuf hblk, htab, hgrp;           // vlscan_hits_stats: per-block bucket + multi-bucket flag, the group table (tags, counts, state), the emitted groups;
-                                           // vlscan_last_rows: per-block keys / weights / counts / offsets, the radix select states, the chosen rows
-    vl::DevBuf lcand;                      // vlscan_last_rows: the candidate rows (timestamp, block, row)
+    vl::DevBuf hit_block, glens, goffs, gtiles, gout, gstat;   // build_hit_list: block of each hit; text_offsets / text_bytes (vlscan_gather_values,
+                                           // hits, last rows, facets): value lengths / offsets, exclusive_scan's tile sums, output staging; the error slot
+    vl::DevBuf ts_vals;                    // decoded timestamps / running sums, 8 bytes per row of the batch (k_time_match, decode_listed_timestamps)
+    vl::DevBuf hblk, htab, hgrp;           // laid out by Carve.  vlscan_hits_stats: per-block bucket + multi-bucket flag, the group table (tags,
+                                           // counts, state), the emitted groups.  vlscan_last_rows: per-block keys / candidate offsets / weights /
+                                           // counts / marks and the candidate and decode lists, the radix select states, the chosen rows.
+                                           // vlscan_facets: hblk the field table, entry bases / cursors, work counter, flag and blocks with hits;
+                                           // hgrp the emitted entries and the string representatives (htab unused)
+    vl::DevBuf lcand;                      // vlscan_last_rows: the candidate rows (timestamp, block, row), laid out by Carve
     vl::DevBuf ftab;                       // vlscan_facets: the per-field tables (tags, counts) and states
     std::vector<vl::DevBuf> ftxt;          // vlscan_facets: per requested field, the texts of every hit when the field is stored as float64 / ipv4 / iso8601
     vl::DevBuf need;                       // bloom-first probe pass: one byte per (block, field), set when the column's values must be staged

@@ -1166,14 +1166,17 @@ static __global__ void __launch_bounds__(256) k_finalize(BatchView B, const uint
 }
 
 // ---- hit-row offsets (bitmap.forEachSetBitReadonly bitmap.go:156-183) ----------------------------------------------------------------------------------
-static __global__ void k_scan_counts(const uint32_t* __restrict__ counts, uint32_t n, uint64_t* __restrict__ offs) {   // single CTA exclusive scan
+// Single CTA exclusive scan of n words into offs[0 .. n), their total into *total.  It also runs in place (in == offs: the tile sums of
+// k_scan_tiles), so no pointer is __restrict__.
+template <typename T>
+static __global__ void k_scan_cta(const T* in, uint32_t n, uint64_t* offs, uint64_t* total) {
     __shared__ uint64_t s[1024];
     __shared__ uint64_t carry;
     if (threadIdx.x == 0) carry = 0;
     __syncthreads();
     for (uint32_t base = 0; base < n; base += blockDim.x) {
-        uint32_t i = base + threadIdx.x;
-        uint64_t v = i < n ? counts[i] : 0;
+        const uint32_t i = base + threadIdx.x;
+        const uint64_t v = i < n ? in[i] : 0;
         s[threadIdx.x] = v;
         __syncthreads();
         for (uint32_t d = 1; d < blockDim.x; d <<= 1) { uint64_t a = threadIdx.x >= d ? s[threadIdx.x - d] : 0; __syncthreads(); s[threadIdx.x] += a; __syncthreads(); }
@@ -1182,24 +1185,7 @@ static __global__ void k_scan_counts(const uint32_t* __restrict__ counts, uint32
         if (threadIdx.x == blockDim.x - 1) carry += s[threadIdx.x];
         __syncthreads();
     }
-    if (threadIdx.x == 0) offs[n] = carry;
-}
-static __global__ void k_hits_compact(BatchView B, const uint64_t* __restrict__ reg, const uint64_t* __restrict__ offs, uint32_t* __restrict__ hits, uint64_t cap) {
-    uint32_t b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (b >= B.nblocks) return;
-    uint64_t lo = B.blk_word_off[b], hi = B.blk_word_off[b + 1];
-    uint64_t out = offs[b];
-    for (uint64_t w0 = lo; w0 < hi; w0 += 32) {
-        uint64_t w = w0 + lane_id();
-        uint64_t bits = w < hi ? reg[w] : 0;
-        uint32_t n = __popcll(bits), incl = n;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, incl, d); if (lane_id() >= d) incl += t; }
-        uint64_t pos = out + incl - n;
-        uint32_t rbase = (uint32_t)(w - lo) * 64;
-        while (bits) { int k = __ffsll((long long)bits) - 1; bits &= bits - 1; if (pos < cap) hits[pos] = rbase + k; pos++; }
-        out += __shfl_sync(0xffffffffu, incl, 31);
-    }
+    if (threadIdx.x == 0) *total = carry;
 }
 
 // ---- timestamps column: encoding.UnmarshalTimestamps on the device (vm/lib/encoding/encoding.go:173-250, nearest_delta2.go:57-90, ------------
@@ -1318,8 +1304,8 @@ static __global__ void __launch_bounds__(256) k_time_match(BatchView B, long lon
 
 // ---- hit materialisation: the selected rows' values and timestamps as blockResult would yield them -------------------------------------------
 // (lib/logstorage/block_result.go:491-507 initTimestampsInternal, :529-591 the per-type readers behind getValues; values_encoder.go:1367-1422)
-// hit h = (hit_block[h], hit_row[h]) in block order, rows ascending (k_hits_compact2).
-static __global__ void k_hits_compact2(BatchView B, const uint64_t* __restrict__ reg, const uint64_t* __restrict__ offs, uint32_t* __restrict__ hits, uint32_t* __restrict__ hit_block, uint64_t cap) {
+// hit h = (hit_block[h], hit_row[h]) in block order, rows ascending (k_hits_compact).
+static __global__ void k_hits_compact(BatchView B, const uint64_t* __restrict__ reg, const uint64_t* __restrict__ offs, uint32_t* __restrict__ hits, uint32_t* __restrict__ hit_block, uint64_t cap) {
     uint32_t b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (b >= B.nblocks) return;
     uint64_t lo = B.blk_word_off[b], hi = B.blk_word_off[b + 1];
@@ -1442,24 +1428,6 @@ static __global__ void __launch_bounds__(256) k_scan_tiles(const uint32_t* __res
     unsigned long long o = tile_sums[blockIdx.x] + pre + incl - sum;
 #pragma unroll
     for (int k = 0; k < 8; k++) { if (base + k < n) offs[base + k] = o; o += x[k]; }
-}
-static __global__ void k_scan_tile_sums(unsigned long long* __restrict__ tile_sums, uint64_t ntiles, unsigned long long* __restrict__ total) {   // single CTA, exclusive, in place
-    __shared__ unsigned long long s[1024];
-    __shared__ unsigned long long carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (uint64_t base = 0; base < ntiles; base += blockDim.x) {
-        const uint64_t i = base + threadIdx.x;
-        const unsigned long long v = i < ntiles ? tile_sums[i] : 0;
-        s[threadIdx.x] = v;
-        __syncthreads();
-        for (uint32_t d = 1; d < blockDim.x; d <<= 1) { unsigned long long a = threadIdx.x >= d ? s[threadIdx.x - d] : 0; __syncthreads(); s[threadIdx.x] += a; __syncthreads(); }
-        if (i < ntiles) tile_sums[i] = carry + s[threadIdx.x] - v;
-        __syncthreads();
-        if (threadIdx.x == blockDim.x - 1) carry += s[threadIdx.x];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *total = carry;
 }
 
 // ---- two-column leaves: eq_field(), le_field() / lt_field() (filter_eq_field.go:60-237, filter_le_field.go:93-313) -------------------------------

@@ -267,6 +267,11 @@ def _b(s):
     return s.encode("utf-8", "surrogateescape") if isinstance(s, str) else bytes(s)
 
 
+def _row_texts(raw, offs, nrows, nf):
+    """rows x fields texts packed into one blob: field f of row i is raw[offs[i * nf + f]:offs[i * nf + f + 1]] -> [tuple of nf bytes] per row"""
+    return [tuple(raw[int(offs[i * nf + f]):int(offs[i * nf + f + 1])] for f in range(nf)) for i in range(nrows)]
+
+
 def _varuint(n):
     out = bytearray()
     while n >= 0x80:
@@ -732,6 +737,16 @@ class Ctx:
         if rc:
             raise VlscanError(rc, lib().vlscan_last_error(self.h).decode("utf-8", "replace"))
 
+    def _call_grown(self, call, caps, needed):
+        """call(*caps) -> (rc, outputs).  A call that fails while needed() reports sizes above its caps runs once more with the caps grown
+        to them.  -> the outputs of the last call; raises its error."""
+        rc, out = call(*caps)
+        want = [int(w) for w in needed()]
+        if rc and any(w > c for w, c in zip(want, caps)):
+            rc, out = call(*[max(c, w) for c, w in zip(caps, want)])
+        self._check(rc)
+        return out
+
     @property
     def stream(self):
         return lib().vlscan_ctx_stream(self.h)
@@ -812,16 +827,12 @@ class Ctx:
         nrows = max(int(batch.rows), 1)
         voffs = np.zeros(nrows + 1, dtype=np.uint64)
         total = C.c_uint64()
-        cap = 1 << 16
-        for _ in range(2):
+
+        def call(cap):
             out = np.zeros(cap, dtype=np.uint8)
-            rc = lib().vlscan_gather_values(self.h, field, C.c_size_t(len(field)), out.ctypes.data_as(C.c_void_p), C.c_uint64(cap), voffs.ctypes.data_as(C.c_void_p), C.c_uint64(nrows),
-                                            C.byref(total), hoffs.ctypes.data_as(C.c_void_p))
-            if rc and total.value > cap:
-                cap = total.value
-                continue
-            self._check(rc)
-            break
+            return lib().vlscan_gather_values(self.h, field, C.c_size_t(len(field)), out.ctypes.data_as(C.c_void_p), C.c_uint64(cap), voffs.ctypes.data_as(C.c_void_p),
+                                              C.c_uint64(nrows), C.byref(total), hoffs.ctypes.data_as(C.c_void_p)), out
+        out = self._call_grown(call, (1 << 16,), lambda: (total.value,))
         n = int(hoffs[-1])
         raw = out.tobytes()
         return [raw[int(voffs[i]):int(voffs[i + 1])] for i in range(n)], hoffs
@@ -833,28 +844,21 @@ class Ctx:
         batch = batch or getattr(self, "_last", None)
         q, keep = hits_query(step, offset, calendar, by)
         nby = len(by)
-        cap_groups, cap_bytes = max(1, min(int(batch.rows) if batch else 0, 1 << 16)), 1 << 16
         out_info = (C.c_uint64 * 4)()
-        for _ in range(2):
+
+        def call(cap_groups, cap_bytes):
             buckets = np.zeros(cap_groups, dtype=np.int64)
             counts = np.zeros(cap_groups, dtype=np.uint64)
             offs = np.zeros(cap_groups * nby + 1, dtype=np.uint64)
             kb = np.zeros(max(cap_bytes, 1), dtype=np.uint8)
             rc = lib().vlscan_hits_stats(self.h, C.byref(q), buckets.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p), C.c_uint64(cap_groups),
                                          kb.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes), offs.ctypes.data_as(C.c_void_p), out_info)
-            if rc and (out_info[0] > cap_groups or out_info[1] > cap_bytes):
-                cap_groups, cap_bytes = max(cap_groups, out_info[0]), max(cap_bytes, out_info[1])
-                continue
-            self._check(rc)
-            break
+            return rc, (buckets, counts, offs, kb)
+        buckets, counts, offs, kb = self._call_grown(call, (max(1, min(int(batch.rows) if batch else 0, 1 << 16)), 1 << 16), lambda: out_info[:2])
         if info is not None:
             info.update(groups=out_info[0], key_bytes=out_info[1], rows=out_info[2], blocks_decoded=out_info[3])
-        raw = kb.tobytes()
-        out = []
-        for g in range(int(out_info[0])):
-            keys = tuple(raw[int(offs[g * nby + f]):int(offs[g * nby + f + 1])] for f in range(nby))
-            out.append((int(buckets[g]), keys, int(counts[g])))
-        return out
+        keys = _row_texts(kb.tobytes(), offs, int(out_info[0]), nby)
+        return [(int(buckets[g]), keys[g], int(counts[g])) for g in range(int(out_info[0]))]
 
     def last_rows(self, limit, fields=(), min_timestamp=None, info=None):
         """The `limit` newest selected rows of the last scan with _time >= min_timestamp (vlscan_last_rows)
@@ -862,9 +866,9 @@ class Ctx:
         value_bytes, selected (rows of the scan) and blocks_decoded (blocks whose timestamps had to be decoded)."""
         q, keep = last_query(limit, fields, min_timestamp)
         nf = len(fields)
-        cap_rows, cap_bytes = max(1, min(int(limit), 1 << 12)), 1 << 16
         out_info = (C.c_uint64 * 4)()
-        for _ in range(2):
+
+        def call(cap_rows, cap_bytes):
             ts = np.zeros(cap_rows, dtype=np.int64)
             blocks = np.zeros(cap_rows, dtype=np.uint32)
             rows = np.zeros(cap_rows, dtype=np.uint32)
@@ -872,19 +876,12 @@ class Ctx:
             vb = np.zeros(max(cap_bytes, 1), dtype=np.uint8)
             rc = lib().vlscan_last_rows(self.h, C.byref(q), ts.ctypes.data_as(C.c_void_p), blocks.ctypes.data_as(C.c_void_p), rows.ctypes.data_as(C.c_void_p),
                                         C.c_uint64(cap_rows), vb.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes), offs.ctypes.data_as(C.c_void_p), out_info)
-            if rc and (out_info[0] > cap_rows or out_info[1] > cap_bytes):
-                cap_rows, cap_bytes = max(cap_rows, out_info[0]), max(cap_bytes, out_info[1])
-                continue
-            self._check(rc)
-            break
+            return rc, (ts, blocks, rows, offs, vb)
+        ts, blocks, rows, offs, vb = self._call_grown(call, (max(1, min(int(limit), 1 << 12)), 1 << 16), lambda: out_info[:2])
         if info is not None:
             info.update(rows=out_info[0], value_bytes=out_info[1], selected=out_info[2], blocks_decoded=out_info[3])
-        raw = vb.tobytes()
-        out = []
-        for i in range(int(out_info[0])):
-            texts = tuple(raw[int(offs[i * nf + f]):int(offs[i * nf + f + 1])] for f in range(nf))
-            out.append((int(ts[i]), int(blocks[i]), int(rows[i]), texts))
-        return out
+        texts = _row_texts(vb.tobytes(), offs, int(out_info[0]), nf)
+        return [(int(ts[i]), int(blocks[i]), int(rows[i]), texts[i]) for i in range(int(out_info[0]))]
 
     def facets(self, fields, max_values_per_field=0, max_value_len=0, info=None):
         """The facets state of the selected rows of the last scan (vlscan_facets) -> {field: None when dropped, else [(class, text as bytes,
@@ -892,9 +889,9 @@ class Ctx:
         `info` (a dict) receives entries, value_bytes, rows (selected) and blocks_decoded (blocks whose timestamps had to be decoded)."""
         q, keep = facets_query(fields, max_values_per_field, max_value_len)
         nf = len(fields)
-        cap_entries, cap_bytes = 1 << 12, 1 << 16
         out_info = (C.c_uint64 * 4)()
-        for _ in range(2):
+
+        def call(cap_entries, cap_bytes):
             dropped = np.zeros(max(nf, 1), dtype=np.uint8)
             foffs = np.zeros(nf + 1, dtype=np.uint64)
             hits = np.zeros(cap_entries, dtype=np.uint64)
@@ -904,11 +901,8 @@ class Ctx:
             rc = lib().vlscan_facets(self.h, C.byref(q), dropped.ctypes.data_as(C.c_void_p), foffs.ctypes.data_as(C.c_void_p), hits.ctypes.data_as(C.c_void_p),
                                      cls.ctypes.data_as(C.c_void_p), C.c_uint64(cap_entries), vb.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes),
                                      voffs.ctypes.data_as(C.c_void_p), out_info)
-            if rc and (out_info[0] > cap_entries or out_info[1] > cap_bytes):
-                cap_entries, cap_bytes = max(cap_entries, out_info[0]), max(cap_bytes, out_info[1])
-                continue
-            self._check(rc)
-            break
+            return rc, (dropped, foffs, hits, cls, voffs, vb)
+        dropped, foffs, hits, cls, voffs, vb = self._call_grown(call, (1 << 12, 1 << 16), lambda: out_info[:2])
         if info is not None:
             info.update(entries=out_info[0], value_bytes=out_info[1], rows=out_info[2], blocks_decoded=out_info[3])
         raw = vb.tobytes()
