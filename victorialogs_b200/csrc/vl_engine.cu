@@ -13,6 +13,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include "vl_copier.h"
 #include "vl_engine.h"
 #include "vl_program.h"
 #include "vl_part.h"
@@ -148,24 +149,271 @@ void finish_batch_layout(vlscan_ctx* ctx, vlscan_batch* b, const std::vector<uin
 // The on-disk values blocks of a batch in (block, column) order; each one's place in the compressed staging buffer is a running sum that
 // starts behind 512 bytes of headroom (the device bit readers load whole aligned words around a stream).  Returns the end of the last one.
 // need (may be NULL = all): need[block * nfields + field] != 0 for the columns whose values are staged (phase 2 of a bloom-first upload).
-static uint64_t collect_values_blocks(const vlscan_block* blocks, uint64_t nblocks, std::vector<ZValuesBlock>& zv, const uint8_t* need = nullptr, uint32_t nfields = 0) {
+// at (may be NULL): at[block * nfields + field] = the index in zv of that cell's block (the first, should a block list the field twice).
+static uint64_t collect_values_blocks(const vlscan_block* blocks, uint64_t nblocks, std::vector<ZValuesBlock>& zv, const uint8_t* need = nullptr, uint32_t nfields = 0, std::vector<size_t>* at = nullptr) {
     uint64_t zc = 512;
+    if (at) at->assign((size_t)nblocks * nfields, SIZE_MAX);
     for (uint64_t b = 0; b < nblocks; b++)
         for (uint32_t k = 0; k < blocks[b].ncols; k++) {
             const vlscan_column& c = blocks[b].cols[k];
             if (c.kind != VLSCAN_COL_VALUES || c.stage != VLSCAN_STAGE_ONDISK) continue;
             if (need && (c.field >= nfields || !need[b * nfields + c.field])) continue;
+            if (at && c.field < nfields && (*at)[b * nfields + c.field] == SIZE_MAX) (*at)[b * nfields + c.field] = zv.size();
             zv.push_back({c.values, (size_t)c.values_len, zc});
             zc += c.values_len;
         }
     return zc;
 }
-// Host threads for the header walk and the descriptor tables of an upload: VLSCAN_HOST_THREADS, else up to 16 (one process per GPU shares the
-// box with its peers).  0 selects the single-threaded block-by-block walk.
-static int host_threads() {
-    if (const char* e = getenv("VLSCAN_HOST_THREADS")) return std::max(0, std::min(256, atoi(e)));
-    return (int)std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
-}
+static double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+
+namespace {
+// One staging step of a batch into one device region (see do_upload).  The helpers below describe cells into the host column table and
+// collect what the region receives; which of them run for which cells is the step's business.  commit() then fills the region.
+struct Upload {
+    vlscan_ctx* ctx; vlscan_batch* out; const vlscan_block* blocks; uint64_t nblocks; uint32_t nfields; vlscan_stats* stats;
+    const std::vector<char>* need_bloom;
+    std::vector<DevColumn>& cols = out->h_cols;   // the steps after the header step continue with the table it left
+    const bool dbg = getenv("VLSCAN_DEBUG_TIMING") != nullptr; const double t_start = now_s();
+    Copier io{ctx};
+    std::vector<uint32_t> rows = std::vector<uint32_t>(nblocks);
+    std::vector<Piece> pieces;   // host -> region
+    std::vector<std::unique_ptr<std::vector<uint8_t>>> owned;   // dict metadata built here
+    uint64_t cursor = 16;   // the first 16 bytes stay unused so that every payload has a readable byte in front of it
+    // On-disk values blocks are not copied into the region: their bytes go to the compressed staging buffer as they are and the device
+    // regenerates them (vl_zstd.cuh) into regions placed behind everything that is copied, so that host memory laid out like
+    // the copied part still goes out as one DMA.  Region offsets are relative to `regen_base` until commit() has sized that part.
+    ZstdJob zjob;
+    uint64_t regen_cursor = 0;
+    struct Ondisk { uint64_t col; uint32_t lens_frame, data_frame; uint64_t lens_rel, data_rel; };
+    std::vector<Ondisk> ondisk;
+    std::vector<OndiskCol> ocols;
+    struct TsFrame { uint64_t block; uint32_t frame; uint64_t rel; };
+    std::vector<TsFrame> ts_frames;
+    std::vector<DevTimestamps> tsv;   // empty until some block comes with its timestamps column
+    // the on-disk values blocks (zv_of: cell -> index in zv / zinfo) and the places of the ZSTD timestamps blocks (by block)
+    std::vector<ZValuesBlock> zv; std::vector<ZValuesInfo> zinfo; std::vector<size_t> zv_of; std::vector<uint64_t> ts_zoff; size_t zbad = SIZE_MAX; std::string zmsg;
+    uint64_t add_piece(const uint8_t* src, uint64_t len) { uint64_t off = arena_reserve(cursor, len); if (len) pieces.push_back({src, len, off}); return off; }
+    // f(block, column, cell) for every column of every block, in order, behind the block's checks and (with `ts`) its timestamps column
+    template <class F> void walk(bool ts, F&& f) {
+        for (uint64_t b = 0; b < nblocks; b++) {
+            const vlscan_block& blk = blocks[b];
+            if (blk.rows > (8u << 20)) throw BadInput("block rows exceed maxRowsPerBlock (8Mi)");   // consts.go:24
+            rows[b] = (uint32_t)blk.rows;
+            if (ts) timestamps(blk, b);
+            for (uint32_t k = 0; k < blk.ncols; k++) {
+                if (blk.cols[k].field >= nfields) throw BadInput("column refers to a field outside the batch field table");
+                f(blk, blk.cols[k], (size_t)b * nfields + blk.cols[k].field);
+            }
+        }
+    }
+    // The compressed bytes of the on-disk values blocks (those marked in `need`, or all) and, with `ts`, of the ZSTD timestamps blocks are
+    // shipped first, so that the DMA engine is busy while the host walks frame and block headers.
+    void sources(const uint8_t* need, bool ts) {
+        uint64_t zc = collect_values_blocks(blocks, nblocks, zv, need, nfields, &zv_of);
+        for (const ZValuesBlock& v : zv) if (v.n) io.src.push_back({v.p, v.n, v.zoff});
+        ts_zoff.resize(ts ? nblocks : 0);
+        for (uint64_t b = 0; b < nblocks && ts; b++) {
+            const vlscan_block& blk = blocks[b];
+            if (blk.ts_marshal_type != MT_ZSTD_NEAREST_DELTA2 && blk.ts_marshal_type != MT_ZSTD_NEAREST_DELTA) continue;
+            if (blk.timestamps_len > vl::part::kMaxTimestampsBlockSize) throw BadInput("timestamps block size cannot exceed 8 MiB");   // getTimestamps block_search.go:490-493
+            ts_zoff[b] = zc;
+            if (blk.timestamps_len) io.src.push_back({blk.timestamps, blk.timestamps_len, zc});
+            zc += blk.timestamps_len;
+        }
+        if (!io.src.empty()) { ctx->zsrc.ensure(zc + 512); io.send_sources(ctx->zsrc.as<uint8_t>()); }
+        // frame, block and section headers of all of them, on several host threads; a malformed block is reported when values() gets to it
+        zinfo.resize(zv.size());
+        const double t_w = now_s();
+        if (!zv.empty()) zjob.add_values_blocks(zv.data(), zv.size(), host_threads(), zinfo.data(), &zbad, &zmsg);
+        if (dbg) fprintf(stderr, "[vlscan upload] header walk of %zu values blocks on %d host threads: %.1f ms (after %.1f ms of collecting and enqueueing the copies)\n",
+                         zv.size(), host_threads(), 1e3 * (now_s() - t_w), 1e3 * (t_w - t_start));
+    }
+    // kind, const value, bloom filter and dict table of a column; `payload` stages or defers the values, whose pieces come before the bloom filter
+    template <class F> void header(const vlscan_column& c, size_t i, F&& payload) {
+        DevColumn& d = cols[i];
+        if (d.kind != COL_MISSING) throw BadInput("duplicate column for one field in a block");
+        if (c.kind == VLSCAN_COL_CONST) {
+            d.kind = COL_CONST; d.meta_len = (uint32_t)c.const_len; d.meta_off = add_piece(c.const_value, c.const_len);
+            return;
+        }
+        if (c.kind != VLSCAN_COL_VALUES) throw BadInput("unknown column kind");
+        if (c.value_type < VT_STRING || c.value_type >= VT_MAX) throw BadInput("unknown valueType");
+        d.kind = COL_VALUES; d.vt = c.value_type; d.min_value = c.min_value; d.max_value = c.max_value;
+        payload();
+        if (c.bloom_len % 8) throw BadInput("cannot unmarshal bloomFilter from src with size not multiple by 8");   // bloomfilter.go:59-61
+        if (need_bloom && !(*need_bloom)[c.field]) { d.bloom_words = 0; d.bloom_off = add_piece(c.bloom, 0); }
+        else { d.bloom_words = (uint32_t)(c.bloom_len / 8); d.bloom_off = add_piece(c.bloom, c.bloom_len); }
+        if (c.value_type == VT_DICT) {
+            if (c.dict_len > 8) throw BadInput("valuesDict may contain max 8 items");
+            d.dict_len = c.dict_len;
+            uint32_t total = c.dict_len ? c.dict_offsets[c.dict_len] : 0;
+            d.meta_len = total;
+            if (c.dict_len && c.dict_blob == (const uint8_t*)c.dict_offsets + 4 * (c.dict_len + 1)) {
+                d.meta_off = add_piece((const uint8_t*)c.dict_offsets, 4 * (c.dict_len + 1) + total);   // caller memory already has the device layout
+            } else {
+                auto meta = std::make_unique<std::vector<uint8_t>>();
+                meta->resize(4 * (c.dict_len + 1) + total);
+                if (c.dict_len) memcpy(meta->data(), c.dict_offsets, 4 * (c.dict_len + 1)); else memset(meta->data(), 0, 4);
+                if (total) memcpy(meta->data() + 4 * (c.dict_len + 1), c.dict_blob, total);
+                d.meta_off = add_piece(meta->data(), meta->size());
+                owned.push_back(std::move(meta));
+            }
+        }
+    }
+    // the values payload of a column: on-disk stage -> regenerated by the device decoder, decoded stage -> copied
+    void values(const vlscan_block& blk, const vlscan_column& c, size_t ci) {
+        DevColumn& d = cols[ci];
+        if (c.stage == VLSCAN_STAGE_ONDISK) {
+            // stringsBlockUnmarshaler.unmarshal: bytesBlock(lens) ++ bytesBlock(data) (encoding.go:83-108).  The host reads the
+            // containers, the frame header and the block headers; the payload is regenerated on the device.
+            const size_t z = zv_of[ci];
+            if (z >= zbad) throw BadInput(zmsg);
+            const uint64_t lens_len = zinfo[z].lens_len, data_len = zinfo[z].data_len;
+            if (data_len > 0xFFFFFFFFull) throw BadInput("values block too large");
+            // the uint block type byte lands on offset 15 of its region, so the lens items behind it are 16-byte aligned
+            const uint64_t lr = arena_reserve(regen_cursor, lens_len + 15), dr = arena_reserve(regen_cursor, data_len);
+            d.lens_off = lr + 16; d.data_off = dr; d.data_len = data_len;
+            ondisk.push_back({ci, (uint32_t)(2 * z), (uint32_t)(2 * z + 1), lr + 15, dr});   // frames 2z, 2z + 1: lens and data
+            ocols.push_back({ci, lens_len, blk.rows});   // lens header checks + lens_type / lens_const / data_const: k_finish_ondisk_cols
+        } else if (c.stage == VLSCAN_STAGE_DECODED) {
+            const uint8_t* lens_items = c.lens_items; const uint64_t lens_len = c.lens_items_len, data_len = c.data_len;
+            // unmarshalUint64Items header checks (encoding.go:246-336)
+            if (lens_len < 1) throw BadInput("cannot unmarshal uint64 block type from empty src");
+            uint8_t lt = lens_items[0];
+            if (lt > 7) throw BadInput("unexpected uint64 block type");
+            uint64_t want = lt < 4 ? (blk.rows << lt) : (1ull << (lt - 4));
+            if (lens_len - 1 != want) throw BadInput("unexpected block length for uint items");
+            d.lens_type = lt;
+            if (lt >= 4) { uint64_t v = 0; for (uint64_t i = 0; i < want; i++) v = (v << 8) | lens_items[1 + i]; if (v > 0xFFFFFFFFull) throw BadInput("row length does not fit 32 bits"); d.lens_const = (uint32_t)v; }
+            if (data_len > 0xFFFFFFFFull) throw BadInput("values block too large");
+            d.lens_off = add_piece(lens_items + 1, lens_len - 1);
+            d.data_off = add_piece(c.data, data_len); d.data_len = data_len;
+            // decode rule of encoding.go:113-120: rows >= 2, all lens equal, len(data) == lens[0] => every row = data
+            d.data_const = (blk.rows >= 2 && lt >= 4 && data_len == d.lens_const) ? 1 : 0;
+        } else throw BadInput("unknown values stage");
+    }
+    // the timestamps column of a block that has one: encoded deltas as stored + timestampsHeader (block_header.go:990-997)
+    void timestamps(const vlscan_block& blk, uint64_t b) {
+        if (!blk.ts_marshal_type) return;
+        if (blk.ts_marshal_type > MT_NEAREST_DELTA) throw BadInput("unknown MarshalType of a timestamps block");
+        if (blk.timestamps_len > vl::part::kMaxTimestampsBlockSize) throw BadInput("timestamps block size cannot exceed 8 MiB");
+        if (tsv.empty()) { tsv.resize(nblocks); memset(tsv.data(), 0, nblocks * sizeof(DevTimestamps)); }
+        DevTimestamps& t = tsv[b];
+        t.first = blk.min_timestamp; t.max = blk.max_timestamp;
+        if (blk.ts_marshal_type == MT_ZSTD_NEAREST_DELTA2 || blk.ts_marshal_type == MT_ZSTD_NEAREST_DELTA) {
+            uint64_t regen = 0; uint32_t id = 0;
+            zjob.add_frame(blk.timestamps, blk.timestamps_len, ts_zoff[b], &regen, &id);   // throws on a malformed frame header
+            if (regen > 10ull * blk.rows + 16) throw BadInput("cannot unmarshal timestamps: the decompressed block is larger than its varints can be");
+            t.mt = blk.ts_marshal_type == MT_ZSTD_NEAREST_DELTA2 ? MT_NEAREST_DELTA2 : MT_NEAREST_DELTA;
+            t.len = (uint32_t)regen;
+            ts_frames.push_back({b, id, arena_reserve(regen_cursor, regen)});
+        } else {
+            t.mt = (uint8_t)blk.ts_marshal_type; t.len = (uint32_t)blk.timestamps_len;
+            t.off = add_piece(blk.timestamps, blk.timestamps_len);
+        }
+    }
+
+    // Places the regenerated regions behind the copied part, sizes `region` and fills it; returns its size.  patch (may be NULL = the whole
+    // column table): the cells of a late region, whose table entries alone are sent.  layout: a new batch, whose layout tables are built too.
+    uint64_t commit(DevBuf& region, const std::vector<uint64_t>* patch, bool layout) {
+        const uint64_t regen_base = (cursor + kArenaAlign - 1) / kArenaAlign * kArenaAlign;
+        for (const Ondisk& o : ondisk) {
+            DevColumn& d = cols[o.col];
+            d.lens_off += regen_base; d.data_off += regen_base;
+            zjob.set_dst(o.lens_frame, regen_base + o.lens_rel); zjob.set_dst(o.data_frame, regen_base + o.data_rel);
+        }
+        for (const TsFrame& tf : ts_frames) { tsv[tf.block].off = regen_base + tf.rel; zjob.set_dst(tf.frame, regen_base + tf.rel); }
+        const bool have_z = !ondisk.empty() || !ts_frames.empty();
+        if (have_z) cursor = regen_base + regen_cursor;
+        const uint64_t bytes = cursor + kArenaPad;
+        const double t_desc = now_s();
+        region.ensure(bytes);
+        const double t_alloc = now_s();
+        // Late cells keep the arena-relative addressing of every kernel: their offsets are taken from the batch arena's base to the late region
+        // (modulo 2^64, so a region below the arena works too), and k_finish_ondisk_cols reads them against that base as well.
+        uint8_t* cols_base = region.as<uint8_t>();
+        std::vector<ColPatch> patches;
+        if (patch) {
+            const uint64_t delta = (uint64_t)(uintptr_t)region.p - (uint64_t)(uintptr_t)out->arena.p;
+            cols_base = out->arena.as<uint8_t>();
+            patches.resize(patch->size());
+            for (size_t i = 0; i < patch->size(); i++) {
+                DevColumn& d = cols[(*patch)[i]];
+                d.lens_off += delta; d.data_off += delta;
+                patches[i].col = (*patch)[i]; patches[i].c = d;
+            }
+        }
+        // the region is cleared on the compute stream; the copy stream takes over from there
+        cudaStream_t cs = ctx->copy_stream;
+        cudaEvent_t ev_cleared = io.events.make(), ev_copied = io.events.make();
+        VL_CUDA(cudaMemsetAsync(region.p, 0, bytes, ctx->stream));
+        VL_CUDA(cudaEventRecord(ev_cleared, ctx->stream));
+        VL_CUDA(cudaStreamWaitEvent(cs, ev_cleared, 0));
+        // The decoder is enqueued BEFORE anything below that can block this thread (packing pageable pieces through the staging ring, copies
+        // from pageable vectors): each launch group then runs as soon as its compressed bytes have landed, beside the DMA of the later ones.
+        const double t_h2d = dbg ? now_s() : 0;
+        double t_zrun = 0;
+        if (have_z) {
+            zjob.set_group_hook([&](uint64_t src_end) { io.wait_sources(ctx->stream, src_end); });
+            zjob.run(ctx, ctx->zsrc.as<uint8_t>(), region.as<uint8_t>());
+            io.ship_sources(UINT64_MAX);
+            if (dbg) t_zrun = now_s();
+        }
+        io.copy(pieces, region.as<uint8_t>());
+        // the column table, or only the entries of a late region's cells: the table on the device has what k_finish_ondisk_cols derived since
+        DevBuf& table = patch ? ctx->patch : out->cols;
+        const void* entries = patch ? (const void*)patches.data() : (const void*)cols.data();
+        const size_t table_bytes = patch ? patches.size() * sizeof(ColPatch) : cols.size() * sizeof(DevColumn);
+        table.ensure(std::max<size_t>(table_bytes, 16));
+        if (table_bytes) VL_CUDA(cudaMemcpyAsync(table.p, entries, table_bytes, cudaMemcpyHostToDevice, cs));
+        io.h2d += table_bytes;
+        if (!patch) out->has_ts = !tsv.empty();   // a late region leaves the timestamps alone
+        if (!tsv.empty()) {
+            out->ts.ensure(nblocks * sizeof(DevTimestamps));
+            VL_CUDA(cudaMemcpyAsync(out->ts.p, tsv.data(), nblocks * sizeof(DevTimestamps), cudaMemcpyHostToDevice, cs));
+            io.h2d += nblocks * sizeof(DevTimestamps);
+        }
+        VL_CUDA(cudaEventRecord(ev_copied, cs));
+        if (!patches.empty()) {
+            VL_CUDA(cudaStreamWaitEvent(ctx->stream, ev_copied, 0));
+            k_patch_cols<<<cdiv(patches.size(), 128), 128, 0, ctx->stream>>>(out->cols.as<DevColumn>(), ctx->patch.as<ColPatch>(), (uint32_t)patches.size());
+            launch_check(ctx);
+        }
+        const double t_enq = dbg ? now_s() : 0;
+        if (have_z) {
+            // the on-disk payloads are being regenerated in HBM; derive lens_type / lens_const / data_const from the regenerated lens blocks
+            VL_CUDA(cudaStreamWaitEvent(ctx->stream, ev_copied, 0));
+            ctx->zcols.ensure(16 + ocols.size() * sizeof(OndiskCol));
+            VL_CUDA(cudaMemsetAsync(ctx->zcols.p, 0, 16, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(ctx->zcols.as<uint8_t>() + 16, ocols.data(), ocols.size() * sizeof(OndiskCol), cudaMemcpyHostToDevice, ctx->stream));
+            if (!ocols.empty()) {
+                k_finish_ondisk_cols<<<cdiv(ocols.size(), 128), 128, 0, ctx->stream>>>(cols_base, out->cols.as<DevColumn>(), (const OndiskCol*)(ctx->zcols.as<uint8_t>() + 16),
+                                                                                         (uint32_t)ocols.size(), ctx->zcols.as<unsigned long long>());
+                launch_check(ctx);
+            }
+            io.h2d += ocols.size() * sizeof(OndiskCol);
+            zjob.check(ctx);   // synchronises the stream
+            unsigned long long cst[2] = {0, 0};
+            VL_CUDA(cudaMemcpy(cst, ctx->zcols.p, 16, cudaMemcpyDeviceToHost));
+            static const char* what[] = {"", "cannot unmarshal uint64 block type from empty src", "unexpected uint64 block type", "unexpected block length for uint items", "row length does not fit 32 bits"};
+            if (cst[0]) throw BadInput(what[std::min<unsigned long long>(cst[0], 4)]);
+        }
+        VL_CUDA(cudaStreamWaitEvent(ctx->stream, ev_copied, 0));
+        double t_copy = 0;
+        if (dbg) { VL_CUDA(cudaStreamSynchronize(ctx->stream)); t_copy = now_s(); }
+        if (nfields) out->note_columns(cols);
+        if (layout) finish_batch_layout(ctx, out, rows);   // synchronises the stream => `owned`, `cols`, staging are safe to drop
+        else VL_CUDA(cudaStreamSynchronize(ctx->stream));  // the layout tables are there since the header step
+        if (dbg) fprintf(stderr, "[vlscan upload] blocks=%llu arena=%.1f MB h2d=%.1f MB pieces=%zu+%zu pinned=%d: describe %.1f ms, alloc %.1f ms, copy %.1f ms (%.1f GB/s), "
+                                 "zstd %llu frames / %llu blocks / %llu sequences: enqueue %.1f ms, decode %.1f ms; layout %.1f ms\n", (unsigned long long)nblocks,
+                         bytes / 1e6, io.h2d / 1e6, pieces.size(), io.src.size(), (int)io.all_pinned, 1e3 * (t_desc - t_start), 1e3 * (t_alloc - t_desc), 1e3 * (t_enq - (t_zrun > 0 ? t_zrun : t_h2d)), io.h2d / 1e9 / std::max(t_copy - t_start, 1e-9),
+                         (unsigned long long)zjob.frames(), (unsigned long long)zjob.compressed_blocks(), (unsigned long long)zjob.sequences(), 1e3 * (t_zrun > 0 ? t_zrun - t_h2d : 0), 1e3 * (t_copy - t_enq), 1e3 * (now_s() - t_copy));
+        if (layout) io.h2d += out->nwords * 12 + nblocks * 12;
+        if (stats) stats->h2d_bytes += io.h2d;
+        return bytes;
+    }
+};
+}  // namespace
 
 // need_bloom (may be NULL = all): per batch field, whether the program that will scan this batch ever probes that field's bloom filters.  A filter
 // nobody probes stays on the host (the reference reads a column's bloom filter lazily, only when a filter asks for it: getBloomFilterForColumn,
@@ -178,416 +426,70 @@ static int host_threads() {
 // `need` (-> batch->arena) and flags the others VALUES_ABSENT.
 // UP_LATE (vlscan_stage_selected on a kept batch) stages the values of the columns marked in `need` into a new region of the batch
 // (batch->late), leaves every other cell as it is and rewrites only the staged cells' entries of the device column table.
+// A failed upload drains both streams before the error leaves it: nothing may still read the caller's buffers.
 enum UploadMode { UP_FULL = 0, UP_HEADERS = 1, UP_VALUES = 2, UP_LATE = 3 };
 static void do_upload(vlscan_ctx* ctx, const char* const* field_names, const size_t* field_name_lens, uint32_t nfields, const vlscan_block* blocks,
                       uint64_t nblocks, vlscan_batch* out, vlscan_stats* stats, const std::vector<char>* need_bloom = nullptr, UploadMode mode = UP_FULL,
                       const uint8_t* need = nullptr, uint64_t* zframes = nullptr) {
     VL_CUDA(cudaSetDevice(ctx->device));
     if (nblocks > 0xFFFFFFF0ull) throw BadInput("too many blocks in one batch");
-    const bool dbg = getenv("VLSCAN_DEBUG_TIMING") != nullptr;
-    auto now = [] { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-    double t_start = now(), t_desc = 0, t_alloc = 0, t_copy = 0;
     out->device = ctx->device; out->nfields = nfields;
-    std::vector<DevColumn>& cols = out->h_cols;   // UP_VALUES and UP_LATE continue with the table UP_HEADERS left
-    const bool values_phase = mode == UP_VALUES || mode == UP_LATE;
-    if (!values_phase) {
+    Upload u{ctx, out, blocks, nblocks, nfields, stats, need_bloom};
+    if (mode == UP_FULL || mode == UP_HEADERS) {   // a new batch: the late regions of the previous one are free
         for (uint32_t f = 0; f < nfields; f++) out->field_names.emplace_back(field_names[f], field_name_lens[f]);
-        cols.assign((size_t)nblocks * std::max<uint32_t>(nfields, 1), DevColumn{});
-        memset(cols.data(), 0, cols.size() * sizeof(DevColumn));
-        out->late_used = 0;   // a new batch: the late regions of the previous one are free
-    } else if (cols.size() != (size_t)nblocks * std::max<uint32_t>(nfields, 1) || !need) throw BadInput("internal: values phase of a bloom-first upload without its header phase");
-    out->split_hdr = mode != UP_FULL;
-    if (mode == UP_LATE && out->late_used == out->late.size()) out->late.emplace_back();
-    DevBuf& arena_buf = mode == UP_HEADERS ? out->harena : mode == UP_LATE ? out->late[out->late_used] : out->arena;
-    std::vector<uint64_t> late_cells;   // UP_LATE: the cells staged by this call
-    std::vector<uint32_t> rows(nblocks);
-    struct Piece { const uint8_t* src; uint64_t len; uint64_t dst; };
-    std::vector<Piece> pieces, zpieces;   // host -> arena, host -> compressed staging (on-disk values blocks)
-    std::vector<std::unique_ptr<std::vector<uint8_t>>> owned;   // dict metadata built here
-    uint64_t cursor = 16;   // the first 16 bytes stay unused so that every payload has a readable byte in front of it
-    auto add_piece = [&](const uint8_t* src, uint64_t len) { uint64_t off = arena_reserve(cursor, len); if (len) pieces.push_back({src, len, off}); return off; };
-    // On-disk values blocks are not copied into the arena: their bytes go to the compressed staging buffer as they are and the device
-    // regenerates them (vl_zstd.cuh) into arena regions placed behind everything that is copied, so that host memory laid out like
-    // the copied part still goes out as one DMA.  Region offsets are relative to `regen_base` until the loop below has sized that part.
-    ZstdJob zjob;
-    uint64_t regen_cursor = 0;
-    struct Ondisk { uint64_t col; uint32_t lens_frame, data_frame; uint64_t lens_rel, data_rel; };
-    std::vector<Ondisk> ondisk;
-    std::vector<OndiskCol> ocols;
-    // copy pieces: runs that are contiguous on both sides (src stride == dst stride) and live in pinned host memory go out as one
-    // cudaMemcpyAsync; everything else is packed through a pinned staging ring.
-    uint64_t h2d = 0;
-    const size_t CH = 64u << 20;
-    uint8_t* stage = nullptr; cudaEvent_t evs[2] = {nullptr, nullptr}; int cur = 0; size_t fill = 0; uint64_t chunk_dst = 0; bool chunk_open = false;
-    uint8_t* dev_base = nullptr;   // destination buffer of the pieces being copied
-    // All host->device payload copies run on the ctx's copy stream; the compute stream picks them up through events.  While the
-    // compressed staging buffer is being filled, `zmarks` records (end offset, event) pairs so that the decoder of a launch group can
-    // start as soon as the bytes of that group have landed, while later bytes are still in flight.
-    cudaStream_t cs = ctx->copy_stream;
-    // every event of this upload lives in `events`: destroyed when the function is left, by return or by exception (a worker that keeps
-    // hitting malformed parts must not leak one event per batch)
-    struct EventBag {
-        std::vector<cudaEvent_t> all;
-        cudaEvent_t make() { cudaEvent_t e; VL_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); all.push_back(e); return e; }
-        ~EventBag() { for (cudaEvent_t e : all) cudaEventDestroy(e); }
-    } events;
-    std::vector<std::pair<uint64_t, cudaEvent_t>> zmarks;
-    bool marking = false;
-    auto mark = [&](uint64_t end_off) { cudaEvent_t e = events.make(); VL_CUDA(cudaEventRecord(e, cs)); zmarks.push_back({end_off, e}); };
-    // Packing pageable memory (a part's mmap()ed files) into the ring is a memcpy, ~10 GB/s on one core and page faults on cold files: the
-    // segments of a chunk are only recorded while the pieces are walked, and copied by all host threads when the chunk is flushed
-    // (each thread takes an equal byte range of the chunk).
-    struct Seg { const uint8_t* src; size_t at, len; };   // src == nullptr: zeros
-    std::vector<Seg> segs;
-    auto pack_chunk = [&](uint8_t* buf, size_t bytes) {
-        const int nt = (int)std::min<size_t>(std::max(1, host_threads()), bytes / (1u << 20) + 1);
-        auto work = [&](int t) {
-            const size_t lo = bytes * (size_t)t / nt, hi = bytes * (size_t)(t + 1) / nt;
-            size_t i = std::upper_bound(segs.begin(), segs.end(), lo, [](size_t v, const Seg& g) { return v < g.at; }) - segs.begin();
-            if (i) i--;
-            for (; i < segs.size() && segs[i].at < hi; i++) {
-                const Seg& g = segs[i];
-                const size_t a = std::max(g.at, lo), b = std::min(g.at + g.len, hi);
-                if (a >= b) continue;
-                if (g.src) memcpy(buf + a, g.src + (a - g.at), b - a); else memset(buf + a, 0, b - a);
-            }
-        };
-        if (nt <= 1) { work(0); return; }
-        if (!ctx->pool) ctx->pool = new HostPool;
-        ctx->pool->run(nt, work);
-    };
-    auto flush = [&]() {
-        if (!chunk_open || !fill) { chunk_open = false; fill = 0; segs.clear(); return; }
-        pack_chunk(stage + (size_t)cur * CH, fill);
-        segs.clear();
-        VL_CUDA(cudaMemcpyAsync(dev_base + chunk_dst, stage + (size_t)cur * CH, fill, cudaMemcpyHostToDevice, cs));
-        VL_CUDA(cudaEventRecord(evs[cur], cs));
-        if (marking) mark(chunk_dst + fill);
-        h2d += fill; cur ^= 1; fill = 0; chunk_open = false;
-        VL_CUDA(cudaEventSynchronize(evs[cur]));
-    };
-    auto is_pinned = [&](const void* p) { cudaPointerAttributes a; if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; } return a.type == cudaMemoryTypeHost; };
-    // Is [p, p + len) inside ONE page-locked allocation?  The runtime API only classifies single addresses; the driver knows the range of the
-    // allocation an address belongs to (cuPointerGetAttribute RANGE_START_ADDR / RANGE_SIZE).  libcuda is always there when a device is.
-    // Pointer queries cost microseconds each and a part's descriptors come as tens of thousands of small pieces (timestamps, const values) out of
-    // the same mmap()ed files: the last answers are remembered.  A 2 MiB-aligned region around a pageable address is taken as pageable as a whole
-    // (if a page-locked allocation begins inside it, its pieces merely take the staging ring), a page-locked allocation by its exact range.
-    uintptr_t pageable_lo = 1, pageable_hi = 0, locked_lo = 1, locked_hi = 0;
-    auto pinned_range_covers = [&](const uint8_t* p, uint64_t len) -> bool {
-        typedef int (*attr_fn)(void*, int, unsigned long long);
-        static const attr_fn fn = [] { void* h = dlopen("libcuda.so.1", RTLD_NOW | RTLD_GLOBAL); return h ? (attr_fn)dlsym(h, "cuPointerGetAttribute") : (attr_fn) nullptr; }();
-        const uintptr_t a = (uintptr_t)p;
-        if (a >= pageable_lo && a < pageable_hi) return false;
-        if (a >= locked_lo && a + len <= locked_hi) return true;
-        if (!is_pinned(p)) { pageable_lo = a & ~(uintptr_t)((2u << 20) - 1); pageable_hi = pageable_lo + (2u << 20); return false; }
-        if (!fn) return len <= 1 || (len <= 4096 && is_pinned(p + len - 1));   // no driver entry point: only what single-address checks can vouch for
-        unsigned long long base = 0; size_t size = 0;
-        if (fn(&base, 11 /* CU_POINTER_ATTRIBUTE_RANGE_START_ADDR */, (unsigned long long)(uintptr_t)p) != 0 || fn(&size, 12 /* CU_POINTER_ATTRIBUTE_RANGE_SIZE */, (unsigned long long)(uintptr_t)p) != 0) return false;
-        if (size) { locked_lo = (uintptr_t)base; locked_hi = (uintptr_t)(base + size); }
-        return (unsigned long long)(uintptr_t)p >= base && (unsigned long long)(uintptr_t)p + len <= base + size;
-    };
-    auto need_stage = [&]() {
-        if (stage) return;
-        stage = (uint8_t*)ctx->ensure_pinned(2 * CH);
-        for (int k = 0; k < 2; k++) { evs[k] = events.make(); VL_CUDA(cudaEventRecord(evs[k], cs)); }
-    };
-    bool all_pinned = true;
-    // pieces [i0, i1) of the list (all of it by default); the staging ring is flushed at the end of every call
-    auto copy_pieces = [&](const std::vector<Piece>& pieces, uint8_t* base, size_t i0 = 0, size_t i1 = SIZE_MAX) {
-    dev_base = base;
-    size_t i = i0;
-    const size_t end = std::min(i1, pieces.size());
-    while (i < end) {
-        // maximal run of pieces laid out identically on both sides (same stride between source and destination)
-        size_t j = i;
-        while (j + 1 < end && pieces[j + 1].src > pieces[j].src && pieces[j + 1].src - pieces[i].src == (ptrdiff_t)(pieces[j + 1].dst - pieces[i].dst)) j++;
-        uint64_t run_len = (pieces[j].dst - pieces[i].dst) + pieces[j].len;
-        // one DMA for the whole run (gaps included) only when the run lies inside a single page-locked allocation: two pinned buffers that
-        // merely line up could have pageable memory between them
-        if (pinned_range_covers(pieces[i].src, run_len)) {
-            // page-locked caller memory: one DMA for the whole run, gaps (alignment slack) included
-            flush();
-            // (split at piece boundaries every ~128 MB so that consumers can be released chunk by chunk)
-            size_t a = i;
-            while (a <= j) {
-                size_t b2 = a;
-                while (b2 < j && (pieces[b2].dst + pieces[b2].len) - pieces[a].dst < (128ull << 20)) b2++;
-                const uint64_t len = (pieces[b2].dst - pieces[a].dst) + pieces[b2].len;
-                VL_CUDA(cudaMemcpyAsync(dev_base + pieces[a].dst, pieces[a].src, len, cudaMemcpyHostToDevice, cs));
-                if (marking) mark(pieces[b2].dst + pieces[b2].len);
-                h2d += len; a = b2 + 1;
-            }
-            (void)run_len;
-            i = j + 1;
-            continue;
+        u.cols.assign((size_t)nblocks * std::max<uint32_t>(nfields, 1), DevColumn{});
+        memset(u.cols.data(), 0, u.cols.size() * sizeof(DevColumn));
+        out->late_used = 0; out->split_hdr = mode == UP_HEADERS;
+    } else if (u.cols.size() != (size_t)nblocks * std::max<uint32_t>(nfields, 1) || !need) throw BadInput("internal: values phase of a bloom-first upload without its header phase");
+    try {
+        switch (mode) {
+        case UP_FULL:
+            u.sources(nullptr, true);
+            u.walk(true, [&](const vlscan_block& blk, const vlscan_column& c, size_t i) { u.header(c, i, [&] { u.values(blk, c, i); }); });
+            out->arena_bytes = u.commit(out->arena, nullptr, true);
+            out->harena_bytes = 0;
+            std::vector<DevColumn>().swap(out->h_cols);   // only a bloom-first upload needs the table again
+            break;
+        case UP_HEADERS:
+            u.walk(false, [&](const vlscan_block&, const vlscan_column& c, size_t i) {
+                u.header(c, i, [&] {
+                    if (c.stage != VLSCAN_STAGE_ONDISK && c.stage != VLSCAN_STAGE_DECODED) throw BadInput("unknown values stage");
+                    u.cols[i].values_state = VALUES_DEFERRED;
+                });
+            });
+            out->harena_bytes = u.commit(out->harena, nullptr, true);
+            break;
+        case UP_VALUES:
+            u.sources(need, true);
+            u.walk(true, [&](const vlscan_block& blk, const vlscan_column& c, size_t i) {
+                if (c.kind != VLSCAN_COL_VALUES) return;
+                u.cols[i].values_state = need[i] ? VALUES_STAGED : VALUES_ABSENT;
+                if (need[i]) u.values(blk, c, i);
+            });
+            out->arena_bytes = u.commit(out->arena, nullptr, false);
+            break;
+        case UP_LATE: {
+            std::vector<uint64_t> staged;
+            u.sources(need, false);
+            u.walk(false, [&](const vlscan_block& blk, const vlscan_column& c, size_t i) {
+                if (c.kind != VLSCAN_COL_VALUES || !need[i]) return;
+                // `need` marks unstaged cells only: one staged already is a field this block lists twice
+                if (u.cols[i].values_state == VALUES_STAGED) throw BadInput("duplicate column for one field in a block");
+                u.cols[i].values_state = VALUES_STAGED;
+                u.values(blk, c, i);
+                staged.push_back(i);
+            });
+            if (out->late_used == out->late.size()) out->late.emplace_back();
+            u.commit(out->late[out->late_used], &staged, false);
+            out->late_used++;
+            *zframes += u.zjob.frames();
+            break;
         }
-        all_pinned = false;
-        need_stage();
-        for (; i <= j; i++) {
-            const Piece& pc = pieces[i];
-            uint64_t done = 0;
-            while (done < pc.len) {
-                if (chunk_open && (chunk_dst + fill != pc.dst + done || fill == CH)) flush();
-                if (!chunk_open) { chunk_open = true; chunk_dst = pc.dst + done; fill = 0; }
-                size_t take = (size_t)std::min<uint64_t>(pc.len - done, CH - fill);
-                segs.push_back({pc.src + done, fill, take});
-                fill += take; done += take;
-            }
-            // pack the space up to the next piece as zeros when it follows closely, so chunks stay large: between two pieces of the copied part
-            // there is nothing but alignment slack and empty reservations (a bloom filter left on the host is 48 bytes of them), zero in the
-            // arena already.  With a 64-byte limit every timestamps block of a part was a chunk, a DMA and an event of its own: 16 k per batch.
-            if (i + 1 < end) {
-                uint64_t gap = pieces[i + 1].dst - (pc.dst + pc.len);
-                if (gap <= 1024 && fill + gap < CH) { if (gap) segs.push_back({nullptr, fill, (size_t)gap}); fill += gap; } else flush();
-            }
         }
+    } catch (...) {
+        cudaStreamSynchronize(ctx->copy_stream); cudaStreamSynchronize(ctx->stream);
+        throw;
     }
-    flush();
-    };
-    // Pre-pass: the compressed bytes of on-disk values blocks are shipped first (their place in the staging buffer is a running sum), so
-    // that the DMA engine is busy while the host walks frame and block headers.
-    bool zlazy = false; size_t zcopied = 0;   // zpieces[0, zcopied) are on their way to the compressed staging buffer
-    auto advance_z = [&](uint64_t limit) {      // enqueue every compressed piece that starts below `limit`
-        size_t hi = zcopied;
-        while (hi < zpieces.size() && zpieces[hi].dst < limit) hi++;
-        if (hi == zcopied) return;
-        marking = true; copy_pieces(zpieces, ctx->zsrc.as<uint8_t>(), zcopied, hi); marking = false;
-        zcopied = hi;
-    };
-    std::vector<ZValuesBlock> zv, zts; std::vector<ZValuesInfo> zinfo; size_t zbad = SIZE_MAX, zo = 0, zt = 0; std::string zmsg;
-    std::vector<DevTimestamps> tsv; bool any_ts = false;
-    struct TsFrame { uint64_t block; uint32_t frame; uint64_t rel; };
-    std::vector<TsFrame> ts_frames;
-    if (mode != UP_HEADERS) {
-        uint64_t zc = collect_values_blocks(blocks, nblocks, zv, values_phase ? need : nullptr, nfields);
-        for (const ZValuesBlock& v : zv) if (v.n) zpieces.push_back({v.p, v.n, v.zoff});
-        // ZSTD-compressed timestamps blocks (marshal types 1 and 4) travel the same way, behind the values blocks (a late call stages none)
-        for (uint64_t b = 0; b < nblocks && mode != UP_LATE; b++) {
-            const vlscan_block& blk = blocks[b];
-            if (blk.ts_marshal_type != MT_ZSTD_NEAREST_DELTA2 && blk.ts_marshal_type != MT_ZSTD_NEAREST_DELTA) continue;
-            if (blk.timestamps_len > vl::part::kMaxTimestampsBlockSize) throw BadInput("timestamps block size cannot exceed 8 MiB");   // getTimestamps block_search.go:490-493
-            zts.push_back({blk.timestamps, (size_t)blk.timestamps_len, zc});
-            if (blk.timestamps_len) zpieces.push_back({blk.timestamps, blk.timestamps_len, zc});
-            zc += blk.timestamps_len;
-        }
-        // Page-locked sources: everything is enqueued right away (asynchronous DMA).  Pageable sources (a part's mmap()ed files) have to be packed
-        // through the staging ring by this thread: that is done lazily, launch group by launch group, from the decoder's group hook below, so
-        // that the device decodes group g while the host packs group g + 1 (packing it all here would finish before the first kernel starts).
-        if (!zpieces.empty()) { ctx->zsrc.ensure(zc + 512); zlazy = !pinned_range_covers(zpieces[0].src, zpieces[0].len); if (!zlazy) advance_z(UINT64_MAX); }
-        // frame, block and section headers of all of them, on several host threads; a malformed block is reported when the loop below gets to it
-        zinfo.resize(zv.size());
-        const double t_w = now();
-        if (!zv.empty()) zjob.add_values_blocks(zv.data(), zv.size(), host_threads(), zinfo.data(), &zbad, &zmsg);
-        if (dbg) fprintf(stderr, "[vlscan upload] header walk of %zu values blocks on %d host threads: %.1f ms (after %.1f ms of collecting and enqueueing the copies)\n",
-                         zv.size(), host_threads(), 1e3 * (now() - t_w), 1e3 * (t_w - t_start));
-    }
-    // the values payload of one column: on-disk stage -> regenerated by the device decoder, decoded stage -> copied
-    auto stage_values = [&](const vlscan_block& blk, const vlscan_column& c, DevColumn& d, uint64_t b) {
-            if (c.stage == VLSCAN_STAGE_ONDISK) {
-                // stringsBlockUnmarshaler.unmarshal: bytesBlock(lens) ++ bytesBlock(data) (encoding.go:83-108).  The host reads the
-                // containers, the frame header and the block headers; the payload is regenerated on the device.
-                if (zo == zbad) throw BadInput(zmsg);
-                const uint64_t lens_len = zinfo[zo].lens_len, data_len = zinfo[zo].data_len;
-                const uint32_t f1 = (uint32_t)(2 * zo), f2 = f1 + 1;
-                zo++;
-                if (data_len > 0xFFFFFFFFull) throw BadInput("values block too large");
-                // the uint block type byte lands on offset 15 of its region, so the lens items behind it are 16-byte aligned
-                const uint64_t lr = arena_reserve(regen_cursor, lens_len + 15), dr = arena_reserve(regen_cursor, data_len);
-                d.lens_off = lr + 16; d.data_off = dr; d.data_len = data_len;
-                const uint64_t ci = (uint64_t)b * nfields + c.field;
-                ondisk.push_back({ci, f1, f2, lr + 15, dr});
-                ocols.push_back({ci, lens_len, blk.rows});   // lens header checks + lens_type / lens_const / data_const: k_finish_ondisk_cols
-            } else if (c.stage == VLSCAN_STAGE_DECODED) {
-                const uint8_t* lens_items = c.lens_items; const uint64_t lens_len = c.lens_items_len, data_len = c.data_len;
-                // unmarshalUint64Items header checks (encoding.go:246-336)
-                if (lens_len < 1) throw BadInput("cannot unmarshal uint64 block type from empty src");
-                uint8_t lt = lens_items[0];
-                if (lt > 7) throw BadInput("unexpected uint64 block type");
-                uint64_t want = lt < 4 ? (blk.rows << lt) : (1ull << (lt - 4));
-                if (lens_len - 1 != want) throw BadInput("unexpected block length for uint items");
-                d.lens_type = lt;
-                if (lt >= 4) { uint64_t v = 0; for (uint64_t i = 0; i < want; i++) v = (v << 8) | lens_items[1 + i]; if (v > 0xFFFFFFFFull) throw BadInput("row length does not fit 32 bits"); d.lens_const = (uint32_t)v; }
-                if (data_len > 0xFFFFFFFFull) throw BadInput("values block too large");
-                d.lens_off = add_piece(lens_items + 1, lens_len - 1);
-                d.data_off = add_piece(c.data, data_len); d.data_len = data_len;
-                // decode rule of encoding.go:113-120: rows >= 2, all lens equal, len(data) == lens[0] => every row = data
-                d.data_const = (blk.rows >= 2 && lt >= 4 && data_len == d.lens_const) ? 1 : 0;
-            } else throw BadInput("unknown values stage");
-    };
-    for (uint64_t b = 0; b < nblocks; b++) {
-        const vlscan_block& blk = blocks[b];
-        if (blk.rows > (8u << 20)) throw BadInput("block rows exceed maxRowsPerBlock (8Mi)");   // consts.go:24
-        rows[b] = (uint32_t)blk.rows;
-        if (blk.ts_marshal_type && (mode == UP_FULL || mode == UP_VALUES)) {   // the timestamps column: encoded deltas as stored + timestampsHeader (block_header.go:990-997)
-            if (blk.ts_marshal_type > MT_NEAREST_DELTA) throw BadInput("unknown MarshalType of a timestamps block");
-            if (blk.timestamps_len > vl::part::kMaxTimestampsBlockSize) throw BadInput("timestamps block size cannot exceed 8 MiB");
-            if (tsv.empty()) { tsv.resize(nblocks); memset(tsv.data(), 0, nblocks * sizeof(DevTimestamps)); }
-            any_ts = true;
-            DevTimestamps& t = tsv[b];
-            t.first = blk.min_timestamp; t.max = blk.max_timestamp;
-            if (blk.ts_marshal_type == MT_ZSTD_NEAREST_DELTA2 || blk.ts_marshal_type == MT_ZSTD_NEAREST_DELTA) {
-                uint64_t regen = 0; uint32_t id = 0;
-                zjob.add_frame(zts[zt].p, zts[zt].n, zts[zt].zoff, &regen, &id);   // throws on a malformed frame header
-                zt++;
-                if (regen > 10ull * blk.rows + 16) throw BadInput("cannot unmarshal timestamps: the decompressed block is larger than its varints can be");
-                t.mt = blk.ts_marshal_type == MT_ZSTD_NEAREST_DELTA2 ? MT_NEAREST_DELTA2 : MT_NEAREST_DELTA;
-                t.len = (uint32_t)regen;
-                ts_frames.push_back({b, id, arena_reserve(regen_cursor, regen)});
-            } else {
-                t.mt = (uint8_t)blk.ts_marshal_type; t.len = (uint32_t)blk.timestamps_len;
-                t.off = add_piece(blk.timestamps, blk.timestamps_len);
-            }
-        }
-        for (uint32_t k = 0; k < blk.ncols; k++) {
-            const vlscan_column& c = blk.cols[k];
-            if (c.field >= nfields) throw BadInput("column refers to a field outside the batch field table");
-            DevColumn& d = cols[(size_t)b * nfields + c.field];
-            if (values_phase) {   // the headers are on the device since phase 1; now the values of the columns the probe pass (or the caller) marked
-                if (c.kind != VLSCAN_COL_VALUES) continue;
-                if (!need[b * nfields + c.field]) { if (mode == UP_VALUES) d.values_state = VALUES_ABSENT; continue; }
-                d.values_state = VALUES_STAGED;
-                stage_values(blk, c, d, b);
-                if (mode == UP_LATE) late_cells.push_back((uint64_t)b * nfields + c.field);
-                continue;
-            }
-            if (d.kind != COL_MISSING) throw BadInput("duplicate column for one field in a block");
-            if (c.kind == VLSCAN_COL_CONST) {
-                d.kind = COL_CONST; d.meta_len = (uint32_t)c.const_len; d.meta_off = add_piece(c.const_value, c.const_len);
-                continue;
-            }
-            if (c.kind != VLSCAN_COL_VALUES) throw BadInput("unknown column kind");
-            if (c.value_type < VT_STRING || c.value_type >= VT_MAX) throw BadInput("unknown valueType");
-            d.kind = COL_VALUES; d.vt = c.value_type; d.min_value = c.min_value; d.max_value = c.max_value;
-            if (mode == UP_HEADERS) {
-                if (c.stage != VLSCAN_STAGE_ONDISK && c.stage != VLSCAN_STAGE_DECODED) throw BadInput("unknown values stage");
-                d.values_state = VALUES_DEFERRED;
-            } else stage_values(blk, c, d, b);
-            if (c.bloom_len % 8) throw BadInput("cannot unmarshal bloomFilter from src with size not multiple by 8");   // bloomfilter.go:59-61
-            if (need_bloom && !(*need_bloom)[c.field]) { d.bloom_words = 0; d.bloom_off = add_piece(c.bloom, 0); }
-            else { d.bloom_words = (uint32_t)(c.bloom_len / 8); d.bloom_off = add_piece(c.bloom, c.bloom_len); }
-            if (c.value_type == VT_DICT) {
-                if (c.dict_len > 8) throw BadInput("valuesDict may contain max 8 items");
-                d.dict_len = c.dict_len;
-                uint32_t total = c.dict_len ? c.dict_offsets[c.dict_len] : 0;
-                d.meta_len = total;
-                if (c.dict_len && c.dict_blob == (const uint8_t*)c.dict_offsets + 4 * (c.dict_len + 1)) {
-                    d.meta_off = add_piece((const uint8_t*)c.dict_offsets, 4 * (c.dict_len + 1) + total);   // caller memory already has the device layout
-                } else {
-                    auto meta = std::make_unique<std::vector<uint8_t>>();
-                    meta->resize(4 * (c.dict_len + 1) + total);
-                    if (c.dict_len) memcpy(meta->data(), c.dict_offsets, 4 * (c.dict_len + 1)); else memset(meta->data(), 0, 4);
-                    if (total) memcpy(meta->data() + 4 * (c.dict_len + 1), c.dict_blob, total);
-                    d.meta_off = add_piece(meta->data(), meta->size());
-                    owned.push_back(std::move(meta));
-                }
-            }
-        }
-    }
-    // regenerated regions follow the copied part
-    const uint64_t regen_base = (cursor + kArenaAlign - 1) / kArenaAlign * kArenaAlign;
-    for (const Ondisk& o : ondisk) {
-        DevColumn& d = cols[o.col];
-        d.lens_off += regen_base; d.data_off += regen_base;
-        zjob.set_dst(o.lens_frame, regen_base + o.lens_rel); zjob.set_dst(o.data_frame, regen_base + o.data_rel);
-    }
-    for (const TsFrame& tf : ts_frames) { tsv[tf.block].off = regen_base + tf.rel; zjob.set_dst(tf.frame, regen_base + tf.rel); }
-    if (!ondisk.empty() || !ts_frames.empty()) cursor = regen_base + regen_cursor;
-    const uint64_t arena_bytes = cursor + kArenaPad;
-    if (mode != UP_LATE) (mode == UP_HEADERS ? out->harena_bytes : out->arena_bytes) = arena_bytes;
-    if (mode == UP_FULL) out->harena_bytes = 0;
-    t_desc = now();
-    arena_buf.ensure(arena_bytes);
-    t_alloc = now();
-    // Late cells keep the arena-relative addressing of every kernel: their offsets are taken from the batch arena's base to the late region
-    // (modulo 2^64, so a region below the arena works too), and k_finish_ondisk_cols reads them against that base as well.
-    uint8_t* cols_base = arena_buf.as<uint8_t>();
-    std::vector<ColPatch> patches;
-    if (mode == UP_LATE) {
-        const uint64_t delta = (uint64_t)(uintptr_t)arena_buf.p - (uint64_t)(uintptr_t)out->arena.p;
-        cols_base = out->arena.as<uint8_t>();
-        patches.resize(late_cells.size());
-        for (size_t i = 0; i < late_cells.size(); i++) {
-            DevColumn& d = cols[late_cells[i]];
-            d.lens_off += delta; d.data_off += delta;
-            patches[i].col = late_cells[i]; patches[i].c = d;
-        }
-    }
-    // the arena is cleared on the compute stream; the copy stream takes over from there
-    cudaEvent_t ev_cleared = events.make(), ev_copied = events.make();
-    VL_CUDA(cudaMemsetAsync(arena_buf.p, 0, arena_bytes, ctx->stream));
-    VL_CUDA(cudaEventRecord(ev_cleared, ctx->stream));
-    VL_CUDA(cudaStreamWaitEvent(cs, ev_cleared, 0));
-    // The decoder is enqueued BEFORE anything below that can block this thread (packing pageable pieces through the staging ring, copies
-    // from pageable vectors): each launch group then runs as soon as its compressed bytes have landed, beside the DMA of the later ones.
-    const bool have_z = !ondisk.empty() || !ts_frames.empty();
-    double t_h2d = 0, t_zrun = 0;
-    if (dbg) t_h2d = now();
-    if (have_z) {
-        zjob.set_group_hook([&](uint64_t src_end) {
-            if (zlazy) advance_z(src_end);
-            for (auto& m : zmarks) if (m.first >= src_end) { VL_CUDA(cudaStreamWaitEvent(ctx->stream, m.second, 0)); return; }
-            if (!zmarks.empty()) VL_CUDA(cudaStreamWaitEvent(ctx->stream, zmarks.back().second, 0));
-        });
-        zjob.run(ctx, ctx->zsrc.as<uint8_t>(), arena_buf.as<uint8_t>());
-        if (zlazy) advance_z(UINT64_MAX);
-        if (dbg) t_zrun = now();
-    }
-    copy_pieces(pieces, arena_buf.as<uint8_t>());
-    if (mode == UP_LATE) {   // only the entries of the cells staged here: the table on the device has what k_finish_ondisk_cols derived since
-        ctx->patch.ensure(std::max<size_t>(patches.size() * sizeof(ColPatch), 16));
-        if (!patches.empty()) VL_CUDA(cudaMemcpyAsync(ctx->patch.p, patches.data(), patches.size() * sizeof(ColPatch), cudaMemcpyHostToDevice, cs));
-        h2d += patches.size() * sizeof(ColPatch);
-    } else {
-        out->cols.ensure(std::max<size_t>(cols.size() * sizeof(DevColumn), 16));
-        if (!cols.empty()) VL_CUDA(cudaMemcpyAsync(out->cols.p, cols.data(), cols.size() * sizeof(DevColumn), cudaMemcpyHostToDevice, cs));
-        h2d += cols.size() * sizeof(DevColumn);
-    }
-    if (mode == UP_FULL || mode == UP_VALUES) out->has_ts = any_ts; else if (mode == UP_HEADERS) out->has_ts = false;
-    if (any_ts) {
-        out->ts.ensure(nblocks * sizeof(DevTimestamps));
-        VL_CUDA(cudaMemcpyAsync(out->ts.p, tsv.data(), nblocks * sizeof(DevTimestamps), cudaMemcpyHostToDevice, cs));
-        h2d += nblocks * sizeof(DevTimestamps);
-    }
-    VL_CUDA(cudaEventRecord(ev_copied, cs));
-    if (!patches.empty()) {
-        VL_CUDA(cudaStreamWaitEvent(ctx->stream, ev_copied, 0));
-        k_patch_cols<<<cdiv(patches.size(), 128), 128, 0, ctx->stream>>>(out->cols.as<DevColumn>(), ctx->patch.as<ColPatch>(), (uint32_t)patches.size());
-        launch_check(ctx);
-    }
-    const double t_enq = dbg ? now() : 0;
-    if (have_z) {
-        // the on-disk payloads are being regenerated in HBM; derive lens_type / lens_const / data_const from the regenerated lens blocks
-        VL_CUDA(cudaStreamWaitEvent(ctx->stream, ev_copied, 0));
-        ctx->zcols.ensure(16 + ocols.size() * sizeof(OndiskCol));
-        VL_CUDA(cudaMemsetAsync(ctx->zcols.p, 0, 16, ctx->stream));
-        VL_CUDA(cudaMemcpyAsync(ctx->zcols.as<uint8_t>() + 16, ocols.data(), ocols.size() * sizeof(OndiskCol), cudaMemcpyHostToDevice, ctx->stream));
-        if (!ocols.empty()) {
-            k_finish_ondisk_cols<<<cdiv(ocols.size(), 128), 128, 0, ctx->stream>>>(cols_base, out->cols.as<DevColumn>(), (const OndiskCol*)(ctx->zcols.as<uint8_t>() + 16),
-                                                                                     (uint32_t)ocols.size(), ctx->zcols.as<unsigned long long>());
-            launch_check(ctx);
-        }
-        h2d += ocols.size() * sizeof(OndiskCol);
-        zjob.check(ctx);   // synchronises the stream
-        unsigned long long cst[2] = {0, 0};
-        VL_CUDA(cudaMemcpy(cst, ctx->zcols.p, 16, cudaMemcpyDeviceToHost));
-        static const char* what[] = {"", "cannot unmarshal uint64 block type from empty src", "unexpected uint64 block type", "unexpected block length for uint items", "row length does not fit 32 bits"};
-        if (cst[0]) throw BadInput(what[std::min<unsigned long long>(cst[0], 4)]);
-    }
-    VL_CUDA(cudaStreamWaitEvent(ctx->stream, ev_copied, 0));
-    if (dbg) { VL_CUDA(cudaStreamSynchronize(ctx->stream)); t_copy = now(); }
-    if (nfields) out->note_columns(cols);
-    if (!values_phase) finish_batch_layout(ctx, out, rows);   // synchronises the stream => `owned`, `cols`, staging are safe to drop
-    else VL_CUDA(cudaStreamSynchronize(ctx->stream));         // the layout tables are there since the header phase
-    if (dbg) fprintf(stderr, "[vlscan upload] blocks=%llu arena=%.1f MB h2d=%.1f MB pieces=%zu+%zu pinned=%d: describe %.1f ms, alloc %.1f ms, copy %.1f ms (%.1f GB/s), "
-                             "zstd %llu frames / %llu blocks / %llu sequences: enqueue %.1f ms, decode %.1f ms; layout %.1f ms\n", (unsigned long long)nblocks,
-                     arena_bytes / 1e6, h2d / 1e6, pieces.size(), zpieces.size(), (int)all_pinned, 1e3 * (t_desc - t_start), 1e3 * (t_alloc - t_desc), 1e3 * (t_enq - (t_zrun > 0 ? t_zrun : t_h2d)), h2d / 1e9 / std::max(t_copy - t_start, 1e-9),
-                     (unsigned long long)zjob.frames(), (unsigned long long)zjob.compressed_blocks(), (unsigned long long)zjob.sequences(), 1e3 * (t_zrun > 0 ? t_zrun - t_h2d : 0), 1e3 * (t_copy - t_enq), 1e3 * (now() - t_copy));
-    (void)all_pinned;
-    if (!values_phase) h2d += out->nwords * 12 + nblocks * 12;
-    if (mode == UP_FULL) std::vector<DevColumn>().swap(out->h_cols);   // only a bloom-first upload needs the table again
-    if (mode == UP_LATE) out->late_used++;
-    if (zframes) *zframes += zjob.frames();
-    if (stats) stats->h2d_bytes += h2d;
 }
 
 // ---- the filter-tree interpreter --------------------------------------------------------------------------------------------
@@ -1010,7 +912,6 @@ int vlscan_batch_upload(vlscan_ctx* ctx, const char* const* field_names, const s
     *out = nullptr;
     auto* b = new vlscan_batch();
     int rc = guarded(ctx, [&] { do_upload(ctx, field_names, field_name_lens, nfields, blocks, nblocks, b, stats); });
-    if (rc) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamSynchronize(ctx->stream); }   // nothing may still read the caller's buffers
     if (rc) { delete b; return rc; }
     *out = b;
     return 0;
@@ -1169,17 +1070,16 @@ int vlscan_zstd_inspect(const void* bytes_block, size_t len, uint64_t out[5]) {
 
 int vlscan_zstd_walk_digest(const vlscan_block* blocks, uint64_t nblocks, int threads, uint64_t out[12]) {
     return guarded(nullptr, [&] {
-        auto now = [] { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
         std::vector<ZValuesBlock> zv;
         collect_values_blocks(blocks, nblocks, zv);
         std::vector<ZValuesInfo> info(zv.size());
         ZstdJob job; size_t bad = SIZE_MAX; std::string msg;
-        const double t0 = now();
+        const double t0 = now_s();
         if (!zv.empty()) job.add_values_blocks(zv.data(), zv.size(), threads, info.data(), &bad, &msg);
-        const double t1 = now();
+        const double t1 = now_s();
         if (bad != SIZE_MAX) throw BadInput("values block " + std::to_string(bad) + ": " + msg);
         job.prepare();
-        const double t2 = now();
+        const double t2 = now_s();
         job.digest(out);
         uint64_t h = 5; for (const ZValuesInfo& x : info) { h = (h ^ x.lens_len) * 0x9E3779B97F4A7C15ull; h = (h ^ x.data_len) * 0x9E3779B97F4A7C15ull; h ^= h >> 29; }
         out[0] ^= h;
@@ -1999,7 +1899,6 @@ static int scan_batch_impl(vlscan_ctx* ctx, const vlscan_program* prog, const ch
             }
         });
     } else rc = guarded(ctx, [&] { do_upload(ctx, field_names, field_name_lens, nfields, blocks, nblocks, b, stats, &need_bloom); });
-    if (rc) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamSynchronize(ctx->stream); }   // nothing may still read the caller's buffers
     if (!rc) rc = vlscan_scan_resident(ctx, prog, b, nullptr);
     if (!rc) rc = vlscan_fetch_results(ctx, out_bitmap_words, out_match_counts, stats);
     if (!rc && stats) {
@@ -2091,8 +1990,7 @@ int vlscan_stage_selected(vlscan_ctx* ctx, const vlscan_block* blocks, uint64_t 
         do_upload(ctx, nullptr, nullptr, nf, blocks, nblocks, b, &st, nullptr, UP_LATE, need.data(), &info[3]);
         info[2] = st.h2d_bytes;
     });
-    if (rc && staging) {   // a half-staged batch is not a result any more; nothing may still read the caller's buffers
-        cudaStreamSynchronize(ctx->copy_stream); cudaStreamSynchronize(ctx->stream);
+    if (rc && staging) {   // a half-staged batch is not a result any more
         ctx->has_result = false; ctx->last_batch = nullptr; ctx->kept = false;
         info[0] = info[1] = info[2] = info[3] = 0;
     }
