@@ -656,8 +656,7 @@ static void read_stats(vlscan_ctx* ctx, vlscan_stats* st, bool check_error) {
     VL_CUDA(cudaStreamSynchronize(ctx->stream));
     if (check_error && h[ST_ERROR]) {
         static const char* const msg[] = {"", "cannot unmarshal strings: row lengths do not add up to the data length", "too big index for dict value",
-                                          "unexpected length for binary representation of a number", "phrase/prefix/regexp over a float64 column needs float->string formatting, which the GPU engine does not implement",
-                                          "unexpected uint64 block type", "the filter needs the timestamps of a block that was handed over without them", "cannot unmarshal timestamps",
+                                          "unexpected length for binary representation of a number", "", "", "the filter needs the timestamps of a block that was handed over without them", "cannot unmarshal timestamps",
                                           "internal: a filter reached the values of a column that the bloom-first probe pass had left on the host"};
         throw BadInput(msg[std::min<unsigned long long>(h[ST_ERROR], 8)]);
     }
@@ -1243,8 +1242,8 @@ static void check_gather_errors(vlscan_ctx* ctx) {
     unsigned long long h[ST_COUNT];
     VL_CUDA(cudaMemcpyAsync(h, ctx->gstat.p, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
     VL_CUDA(cudaStreamSynchronize(ctx->stream));
-    static const char* const msg[] = {"", "cannot unmarshal strings: row lengths do not add up to the data length", "too big index for dict value", "unexpected length for binary representation of a number", "",
-                                      "unexpected uint64 block type", "the timestamps of a block with selected rows were not handed over", "cannot unmarshal timestamps",
+    static const char* const msg[] = {"", "cannot unmarshal strings: row lengths do not add up to the data length", "too big index for dict value", "unexpected length for binary representation of a number", "", "",
+                                      "the timestamps of a block with selected rows were not handed over", "cannot unmarshal timestamps",
                                       "the values of a cell with selected rows are not on the device (vlscan_stage_selected stages them)",
                                       "the decoded timestamps of a block contradict the minimum / maximum of its header"};
     if (h[ST_ERROR]) throw BadInput(msg[std::min<unsigned long long>(h[ST_ERROR], 9)]);
@@ -1286,9 +1285,10 @@ static int field_slot(const vlscan_batch* b, const std::string& name) {
     for (uint32_t s = 0; s < b->nfields; s++) if (b->field_names[s] == name) return (int)s;
     return -1;
 }
-// row offsets of the strings blocks with hits in column `slot` (kept from the scan where it already computed them); `with_rows` (default: the
-// scan's counts) != 0 marks the blocks whose offsets are needed.  On a kept batch every such block must have the field's values on the
-// device: the call fails naming the field otherwise (the kernels would report ERR_VALUES_ABSENT, which cannot say which field it was).
+// row offsets of the blocks with hits whose cell in column `slot` has per-row lens items (cell_needs_offsets; kept from the scan where it already
+// computed them); `with_rows` (default: the scan's counts) != 0 marks the blocks whose offsets are needed.  On a kept batch every such block
+// must have the field's values on the device: the call fails naming the field otherwise (the kernels would report ERR_VALUES_ABSENT, which
+// cannot say which field it was).
 static const uint32_t* hit_row_offsets(vlscan_ctx* ctx, int slot, const std::string& name, const uint32_t* with_rows = nullptr) {
     if (slot < 0) return nullptr;
     BatchView B = ctx->last_batch->view();

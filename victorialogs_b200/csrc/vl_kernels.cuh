@@ -17,7 +17,8 @@ struct DevProgram {
 
 // stats slots (device u64 array)
 enum { ST_VALUES_BYTES = 0, ST_BLOOM_BYTES, ST_COLUMNS_READ, ST_BITMAP_BYTES, ST_ROWS_MATCHED, ST_BLOCKS_MATCHED, ST_ERROR, ST_SCAN_BYTES, ST_COUNT };
-enum { ERR_NONE = 0, ERR_LENS_MISMATCH = 1, ERR_DICT_INDEX = 2, ERR_BAD_WIDTH = 3, ERR_UNSUPPORTED_FLOAT_TOSTRING = 4, ERR_BAD_LENS_TYPE = 5, ERR_NO_TIMESTAMPS = 6, ERR_BAD_TIMESTAMPS = 7, ERR_VALUES_ABSENT = 8,
+// atomicMax keeps the largest code: the numbers rank the errors (4 and 5 are unused)
+enum { ERR_NONE = 0, ERR_LENS_MISMATCH = 1, ERR_DICT_INDEX = 2, ERR_BAD_WIDTH = 3, ERR_NO_TIMESTAMPS = 6, ERR_BAD_TIMESTAMPS = 7, ERR_VALUES_ABSENT = 8,
        ERR_TS_HEADER = 9 };   // decoded timestamps outside the [min, max] of their block header (k_last_rows)
 
 struct BatchView {
@@ -42,6 +43,8 @@ static __device__ __forceinline__ uint32_t width_of_vt(uint32_t vt) {
 static __device__ __forceinline__ uint64_t lens_stored_bytes(const DevColumn& c, uint32_t rows) {
     return 1 + (c.lens_type < 4 ? ((uint64_t)rows << c.lens_type) : (1ull << (c.lens_type - 4)));
 }
+// a values cell whose rows are found through k_lens_offsets: per-row lens items, and not every row the whole payload (encoding.go:113-120)
+static __device__ __forceinline__ bool cell_needs_offsets(const DevColumn& c) { return c.kind == COL_VALUES && c.lens_type < 4 && !c.data_const; }
 // length of row r (unmarshalUint64Items lib/logstorage/encoding.go:246-336)
 static __device__ __forceinline__ uint32_t row_len(const DevColumn& c, const uint8_t* lens, uint32_t r) {
     switch (c.lens_type) {
@@ -1322,15 +1325,13 @@ static __global__ void k_hits_compact(BatchView B, const uint64_t* __restrict__ 
         out += __shfl_sync(0xffffffffu, incl, 31);
     }
 }
-// blocks with hits -> work list: mode 0 = into the lens list those whose column `slot` is a strings column with per-row lens items, mode 1 = into
-// the row list every block with hits (timestamps decode)
+// blocks with hits -> work list: mode 0 = into the lens list those whose cell in column `slot` needs row offsets (cell_needs_offsets), mode 1 =
+// into the row list every block with hits (timestamps decode)
 static __global__ void k_hit_blocks_list(BatchView B, const uint32_t* __restrict__ counts, int slot, int mode, uint32_t* __restrict__ list, uint32_t* __restrict__ work_count) {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B.nblocks || counts[b] == 0) return;
     if (mode == 0) {
-        if (slot < 0) return;
-        const DevColumn& c = B.cols[(uint64_t)b * B.nfields + slot];
-        if (c.kind != COL_VALUES || c.vt != VT_STRING || c.lens_type >= 4 || c.data_const) return;
+        if (slot < 0 || !cell_needs_offsets(B.cols[(uint64_t)b * B.nfields + slot])) return;
         list[atomicAdd(&work_count[WC_LENS], 1u)] = b;
     } else list[atomicAdd(&work_count[WC_ROW], 1u)] = b;
 }
@@ -1349,62 +1350,78 @@ static __global__ void k_gather_ts(BatchView B, const uint32_t* __restrict__ hit
     const uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (h < nhits) out[h] = (long long)ts_vals[B.blk_word_off[hit_block[h]] * 64 + hits[h]];
 }
-// The bytes of a const, strings or dict cell in row r of block b (a column of another kind: none); false for a typed column, whose text
-// must be formatted.  The decode value_text and the facets kernels share.  A values cell whose payload is not on the device (a kept batch
-// before vlscan_stage_selected) reads as no bytes and reports ERR_VALUES_ABSENT.
-static __device__ __forceinline__ bool cell_bytes(const BatchView& B, const DevColumn& c, uint32_t b, uint32_t r, const uint32_t* __restrict__ row_off8, const uint8_t** out,
-                                                  uint32_t* out_len, unsigned long long* __restrict__ stats) {
-    const uint8_t* src = nullptr; uint32_t len = 0; unsigned err = ERR_NONE;   // one error report for every path
-    if (c.kind == COL_CONST) { src = B.hdr + c.meta_off; len = c.meta_len; }
-    else if (c.kind == COL_VALUES) {
-        const uint8_t* data = B.arena + c.data_off;
-        if (c.values_state != VALUES_STAGED) err = ERR_VALUES_ABSENT;
-        else if (c.vt == VT_STRING) {
-            if (c.data_const) { src = data; len = (uint32_t)c.data_len; }
-            else if (c.lens_type >= 4) { len = c.lens_const; src = data + (uint64_t)r * len; }
-            else {
-                const uint8_t* lens = B.arena + c.lens_off;
-                uint32_t o = row_off8[(B.blk_word_off[b] << 3) + (r >> 3)];
-                for (uint32_t q = r & ~7u; q < r; q++) o += row_len(c, lens, q);
-                len = row_len(c, lens, r); src = data + o;
-            }
-            if ((uint64_t)(src - data) + len > c.data_len) { len = 0; err = ERR_LENS_MISMATCH; }
-        } else if (c.vt == VT_DICT) {
-            const uint32_t id = data[r];
-            if (id >= c.dict_len) err = ERR_DICT_INDEX;
-            else { const uint32_t* dof = (const uint32_t*)(B.hdr + c.meta_off); src = B.hdr + c.meta_off + 4 * (c.dict_len + 1) + dof[id]; len = dof[id + 1] - dof[id]; }
-        } else return false;
+// ---- the reader of one cell: row r of a column in block b as blockResultColumn.getValues yields it -----------------------------------------------
+// Three layers: the encoded bytes of a values cell (cell_raw), its text without formatting (cell_text_raw), its text (cell_text).  Each returns
+// an ERR_* code and raises nothing: its caller reports the code with one atomicMax.  row_off8: k_lens_offsets of the cell's slot, built for
+// every block with hits whose cell has per-row lens items (cell_needs_offsets).
+static __device__ __forceinline__ bool cell_typed(const DevColumn* c) { return c && c->kind == COL_VALUES && c->vt != VT_STRING && c->vt != VT_DICT; }
+static __device__ __forceinline__ const DevColumn* cell_at(const BatchView& B, int slot, uint32_t b) { return slot >= 0 ? &B.cols[(uint64_t)b * B.nfields + slot] : nullptr; }
+static __device__ __forceinline__ void report_error(unsigned long long* stats, uint32_t err) { if (err) atomicMax(&stats[ST_ERROR], (unsigned long long)err); }
+// The encoded bytes of row r of a values cell: the whole payload when every row is that one value (rows >= 2, const lens equal to the data
+// length, encoding.go:113-120), else the row's slice by its const or per-row lens item.  A payload that is not on the device (a kept batch
+// before vlscan_stage_selected) is ERR_VALUES_ABSENT.
+static __device__ __forceinline__ uint32_t cell_raw(const BatchView& B, const DevColumn& c, uint32_t b, uint32_t r, const uint32_t* __restrict__ row_off8, const uint8_t** p, uint32_t* n) {
+    if (c.values_state != VALUES_STAGED) return ERR_VALUES_ABSENT;
+    uint64_t off = 0; uint32_t len;
+    if (c.data_const) len = (uint32_t)c.data_len;
+    else if (c.lens_type >= 4) { len = c.lens_const; off = (uint64_t)r * len; }
+    else {
+        const uint8_t* lens = B.arena + c.lens_off;
+        uint32_t o = row_off8[(B.blk_word_off[b] << 3) + (r >> 3)];
+        for (uint32_t q = r & ~7u; q < r; q++) o += row_len(c, lens, q);
+        off = o; len = row_len(c, lens, r);
     }
-    if (err) atomicMax(&stats[ST_ERROR], (unsigned long long)err);
-    *out = src; *out_len = len;
-    return true;
+    if (off + len > c.data_len) return ERR_LENS_MISMATCH;
+    *p = B.arena + c.data_off + off; *n = len;
+    return ERR_NONE;
 }
-// The value of column `slot` (-1: a field the batch lacks) in row r of block b as blockResultColumn.getValues yields it: row bytes of a strings
-// column, the dictionary entry, the text form of a typed value (formatted into buf, VL_FMT_F64_MAX bytes), the const value, "" for a field the
-// block does not have.  row_off8: k_lens_offsets of the slot (strings columns with per-row lens items).  Returns the length, *out the bytes.
-static __device__ uint32_t value_text(const BatchView& B, int slot, uint32_t b, uint32_t r, const uint32_t* __restrict__ row_off8, uint8_t* buf, const uint8_t** out,
-                                      unsigned long long* __restrict__ stats) {
-    const uint8_t* src = nullptr; uint32_t len = 0;
-    if (slot >= 0) {
-        const DevColumn& c = B.cols[(uint64_t)b * B.nfields + slot];
-        if (!cell_bytes(B, c, b, r, row_off8, &src, &len, stats)) {
-            const uint32_t w = width_of_vt(c.vt);
-            const uint64_t raw = load_fixed_be(B.arena + c.data_off + (uint64_t)r * w, w);
-            const int n = c.vt == VT_FLOAT64 ? fmt_f64(buf, raw) : encoded_to_string(c.vt, raw, buf);
-            src = buf; len = n > 0 ? (uint32_t)n : 0;
+// The text of row r without formatting: "" for a field the block does not have (c NULL: no block of the batch has it), the const value, the
+// row bytes of a strings cell, the dictionary entry; for a typed cell (cell_typed) the encoded value, whose text is left to the caller.  A dict
+// or typed value whose length is not its type's width is ERR_BAD_WIDTH.  On an error the text is "".  One exit: with one return per case the
+// facets pass outgrew its registers and spilled.
+static __device__ __forceinline__ uint32_t cell_text_raw(const BatchView& B, const DevColumn* c, uint32_t b, uint32_t r, const uint32_t* __restrict__ row_off8, const uint8_t** p,
+                                                         uint32_t* n) {
+    const uint8_t* src = nullptr; uint32_t len = 0, err = ERR_NONE;
+    if (c && c->kind == COL_CONST) { src = B.hdr + c->meta_off; len = c->meta_len; }
+    else if (c && c->kind == COL_VALUES) {
+        err = cell_raw(B, *c, b, r, row_off8, &src, &len);
+        if (!err && c->vt != VT_STRING && len != width_of_vt(c->vt)) err = ERR_BAD_WIDTH;
+        if (!err && c->vt == VT_DICT) {
+            const uint32_t id = src[0];
+            if (id >= c->dict_len) err = ERR_DICT_INDEX;
+            else { const uint32_t* dof = (const uint32_t*)(B.hdr + c->meta_off); src = B.hdr + c->meta_off + 4 * (c->dict_len + 1) + dof[id]; len = dof[id + 1] - dof[id]; }
         }
+        if (err) len = 0;
     }
-    *out = src;
-    return len;
+    *p = src; *n = len;
+    return err;
 }
-// The value of column `slot` in one row as a string.  pass 0: lens[h] = its length; pass 1: the bytes go to out + offs[h].
+// The text of row r: cell_text_raw with a typed value formatted into buf (VL_FMT_F64_MAX bytes).  Not inlined: inlined, it made the hits and
+// two-column kernels spill more.
+static __device__ __noinline__ uint32_t cell_text(const BatchView& B, const DevColumn* c, uint32_t b, uint32_t r, const uint32_t* __restrict__ row_off8, uint8_t* buf, const uint8_t** p, uint32_t* n) {
+    const uint32_t err = cell_text_raw(B, c, b, r, row_off8, p, n);
+    if (!err && cell_typed(c)) {
+        const uint64_t raw = load_fixed_be(*p, *n);
+        const int k = c->vt == VT_FLOAT64 ? fmt_f64(buf, raw) : encoded_to_string(c->vt, raw, buf);
+        *p = buf; *n = k > 0 ? (uint32_t)k : 0;
+    }
+    return err;
+}
+// The dict ids of a cell in the plain layout, one byte per row (const lens 1, rows bytes of data), which the dict fast paths read directly;
+// NULL for any other cell, whose rows go through the reader.
+static __device__ __forceinline__ const uint8_t* plain_dict_ids(const BatchView& B, const DevColumn& c, uint32_t rows) {
+    const bool plain = c.kind == COL_VALUES && c.vt == VT_DICT && c.values_state == VALUES_STAGED && c.lens_type >= 4 && c.lens_const == 1 && c.data_len == rows && !c.data_const;
+    return plain ? B.arena + c.data_off : nullptr;
+}
+// The value of column `slot` (-1: a field the batch lacks) in one row as a string.  pass 0: lens[h] = its length; pass 1: the bytes go to out + offs[h].
 static __global__ void k_gather_values(BatchView B, int slot, const uint32_t* __restrict__ hits, const uint32_t* __restrict__ hit_block, uint64_t nhits, const uint32_t* __restrict__ row_off8,
                                        int pass, uint32_t* __restrict__ lens_out, const uint64_t* __restrict__ offs, uint8_t* __restrict__ out, unsigned long long* __restrict__ stats) {
     const uint64_t h = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (h >= nhits) return;
     uint8_t buf[VL_FMT_F64_MAX];
-    const uint8_t* src;
-    const uint32_t len = value_text(B, slot, hit_block[h], hits[h], row_off8, buf, &src, stats);
+    const uint8_t* src; uint32_t len;
+    const uint32_t b = hit_block[h];
+    report_error(stats, cell_text(B, cell_at(B, slot, b), b, hits[h], row_off8, buf, &src, &len));
     if (pass == 0) { lens_out[h] = len; return; }
     uint8_t* d = out + offs[h];
     for (uint32_t k = 0; k < len; k++) d[k] = src[k];
@@ -1431,42 +1448,6 @@ static __global__ void __launch_bounds__(256) k_scan_tiles(const uint32_t* __res
 }
 
 // ---- two-column leaves: eq_field(), le_field() / lt_field() (filter_eq_field.go:60-237, filter_le_field.go:93-313) -------------------------------
-// the encoded bytes of row r of a values column (strings: the row; typed: the fixed-width value; dict: the id byte); false when the lens items are off
-static __device__ bool row_bytes(const BatchView& B, const DevColumn& c, uint32_t b, uint32_t r, const uint32_t* __restrict__ row_off8, const uint8_t** p, uint32_t* n) {
-    const uint8_t* data = B.arena + c.data_off;
-    if (c.data_const) { *p = data; *n = (uint32_t)c.data_len; return true; }
-    uint64_t off; uint32_t len;
-    if (c.lens_type >= 4) { len = c.lens_const; off = (uint64_t)r * len; }
-    else {
-        const uint8_t* lens = B.arena + c.lens_off;
-        uint32_t o = row_off8[(B.blk_word_off[b] << 3) + (r >> 3)];
-        for (uint32_t q = r & ~7u; q < r; q++) o += row_len(c, lens, q);
-        off = o; len = row_len(c, lens, r);
-    }
-    if (off + len > c.data_len) return false;
-    *p = data + off; *n = len;
-    return true;
-}
-// the string form of a row's value as blockResult.getValues yields it: const value, "" for a missing field, dict entry, row bytes, text of a typed value
-static __device__ bool row_string(const BatchView& B, const DevColumn* c, uint32_t b, uint32_t r, const uint32_t* __restrict__ row_off8, uint8_t* buf, const uint8_t** p, uint32_t* n) {
-    *p = buf; *n = 0;
-    if (!c || c->kind == COL_MISSING) return true;
-    if (c->kind == COL_CONST) { *p = B.hdr + c->meta_off; *n = c->meta_len; return true; }
-    const uint8_t* v; uint32_t vn;
-    if (!row_bytes(B, *c, b, r, row_off8, &v, &vn)) return false;
-    if (c->vt == VT_STRING) { *p = v; *n = vn; return true; }
-    if (c->vt == VT_DICT) {
-        if (vn != 1 || v[0] >= c->dict_len) return false;
-        const uint32_t* dof = (const uint32_t*)(B.hdr + c->meta_off);
-        *p = B.hdr + c->meta_off + 4 * (c->dict_len + 1) + dof[v[0]]; *n = dof[v[0] + 1] - dof[v[0]];
-        return true;
-    }
-    if (vn != width_of_vt(c->vt)) return false;
-    const uint64_t raw = load_fixed_be(v, vn);
-    const int k = c->vt == VT_FLOAT64 ? fmt_f64(buf, raw) : encoded_to_string(c->vt, raw, buf);
-    *n = k > 0 ? (uint32_t)k : 0;
-    return true;
-}
 // leValuesString filter_le_field.go:283-297: numbers when both sides are numbers, else strings (bytewise, the shorter first on a tie)
 static __device__ bool le_values_string(const uint8_t* a, uint32_t an, const uint8_t* b2, uint32_t bn, bool excl) {
     const double fa = mn::parse_math_number(a, an);
@@ -1515,8 +1496,8 @@ static __global__ void __launch_bounds__(256) k_plan_pair(DevProgram P, BatchVie
         }
         if (act == ACT_PAIR) {
             unsigned long long vb = 0, cols = 0;
-            if (vala) { vb += lens_stored_bytes(*ca, B.blk_rows[b]) + ca->data_len; cols++; if (ca->lens_type < 4 && !ca->data_const) lens_a[atomicAdd(&work_count[WC_LENS], 1u)] = b; }
-            if (valb) { vb += lens_stored_bytes(*cb, B.blk_rows[b]) + cb->data_len; cols++; if (cb->lens_type < 4 && !cb->data_const) lens_b[atomicAdd(&work_count[WC_LENS2], 1u)] = b; }
+            if (vala) { vb += lens_stored_bytes(*ca, B.blk_rows[b]) + ca->data_len; cols++; if (cell_needs_offsets(*ca)) lens_a[atomicAdd(&work_count[WC_LENS], 1u)] = b; }
+            if (valb) { vb += lens_stored_bytes(*cb, B.blk_rows[b]) + cb->data_len; cols++; if (cell_needs_offsets(*cb)) lens_b[atomicAdd(&work_count[WC_LENS2], 1u)] = b; }
             row_blocks[atomicAdd(&work_count[WC_ROW], 1u)] = b;
             atomicAdd(&stats[ST_VALUES_BYTES], vb); atomicAdd(&stats[ST_COLUMNS_READ], cols);
         }
@@ -1529,17 +1510,22 @@ static __device__ __noinline__ bool pair_match_row(const DevProgram& P, const Ba
     const bool le = L.kind == F_LE_FIELD, excl = L.pair_excl != 0;
     const uint8_t *x, *y; uint32_t xn, yn;
     if (mode == PAIR_BINARY) {
-        if (!row_bytes(B, *ca, b, r, ro_a, &x, &xn) || !row_bytes(B, *cb, b, r, ro_b, &y, &yn)) { atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_LENS_MISMATCH); return false; }
+        uint32_t err = cell_raw(B, *ca, b, r, ro_a, &x, &xn);
+        if (!err) err = cell_raw(B, *cb, b, r, ro_b, &y, &yn);
+        if (err) { report_error(stats, err); return false; }
         if (!le) return bytes_equal(x, xn, y, yn);                                        // applyFilterBinValue: same type, same binary form
         if (ca->vt == VT_INT64 && xn == 8 && yn == 8) { const int64_t u = unzigzag64(ld_be64(x)), v = unzigzag64(ld_be64(y)); return excl ? u < v : u <= v; }
         if (ca->vt == VT_FLOAT64 && xn == 8 && yn == 8) { const double u = __longlong_as_double((long long)ld_be64(x)), v = __longlong_as_double((long long)ld_be64(y)); return excl ? u < v : u <= v; }
         return le_values_string(x, xn, y, yn, excl);   // uintN, ipv4, iso8601: their big-endian encodings go through leValuesString as they are (:246-252)
     }
     uint8_t bufa[VL_FMT_F64_MAX], bufb[VL_FMT_F64_MAX];
-    if (!row_string(B, ca, b, r, ro_a, bufa, &x, &xn) || !row_string(B, cb, b, r, ro_b, bufb, &y, &yn)) { atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_DICT_INDEX); return false; }
+    uint32_t err = cell_text(B, ca, b, r, ro_a, bufa, &x, &xn);
+    if (!err) err = cell_text(B, cb, b, r, ro_b, bufb, &y, &yn);
+    if (err) { report_error(stats, err); return false; }
     return le ? le_values_string(x, xn, y, yn, excl) : bytes_equal(x, xn, y, yn);   // PAIR_DICT compares the entries, PAIR_STRINGS the string forms: same code
 }
-static __global__ void __launch_bounds__(256) k_row_pair(DevProgram P, BatchView B, uint32_t leaf_idx, int slot_a, int slot_b, const uint32_t* __restrict__ row_blocks, const uint32_t* __restrict__ work_count,
+// three CTAs per SM: left to itself ptxas gives the reader's call chain 128 registers and the kernel two, which measured slower
+static __global__ void __launch_bounds__(256, 3) k_row_pair(DevProgram P, BatchView B, uint32_t leaf_idx, int slot_a, int slot_b, const uint32_t* __restrict__ row_blocks, const uint32_t* __restrict__ work_count,
                                                           const uint64_t* __restrict__ payload, const uint64_t* __restrict__ reg, const uint32_t* __restrict__ ro_a, const uint32_t* __restrict__ ro_b,
                                                           uint64_t* __restrict__ leaf_bm, unsigned long long* __restrict__ stats) {
     const uint32_t nwork = work_count[WC_ROW];
@@ -1578,7 +1564,7 @@ static __global__ void k_bitmap_digest(BatchView B, const uint64_t* __restrict__
 
 // ---- `stats by (_time:step offset off, f1, ...) count()` over the selected rows: the aggregation of /select/logsql/hits --------------------------
 // (app/vlselect/logsql/logsql.go:116-219 builds it, lib/logstorage/block_result.go:760-848 buckets `_time`).  A group is (bucket, the text of every
-// by-field as value_text yields it).  Groups live in an open-addressing table whose slot holds only a 64-bit tag: the high half of the key's hash
+// by-field as cell_text yields it).  Groups live in an open-addressing table whose slot holds only a 64-bit tag: the high half of the key's hash
 // and 1 + the index of a representative hit.  A key is found by comparing the bucket and the texts with the representative's, byte for byte,
 // so two keys share a slot only when they are equal: a hash collision costs a probe, never a wrong count.  A hit insert that would claim a slot
 // beyond the table's load limit raises the overflow flag; the host then grows the table and runs the pass again.
@@ -1617,12 +1603,47 @@ static __device__ __forceinline__ int64_t hit_bucket(const BatchView& B, const H
     return V.blk_multi[b] ? truncate_timestamp((int64_t)V.ts_vals[B.blk_word_off[b] * 64 + r], q.step, q.offset, q.calendar) : (int64_t)V.blk_bucket[b];
 }
 static __device__ __forceinline__ uint64_t mix64(uint64_t z) { z ^= z >> 30; z *= 0xBF58476D1CE4E5B9ULL; z ^= z >> 27; z *= 0x94D049BB133111EBULL; return z ^ (z >> 31); }
+// The key tables of the hits and the facets: open addressing, a slot holds a count and a 64-bit tag, the high half of the key's hash and 1 + the
+// index of a representative hit (0: empty).  key_table_add adds c to the slot of the key of hit `rep`: a slot whose hash half matches holds the
+// key only when same(its representative) says so, so a hash collision costs a probe, never a wrong count; an empty slot is claimed by CAS when
+// may_claim() allows it.  The caller's policy acts on the outcome.
+enum { KEY_FOUND = 0, KEY_CLAIMED = 1, KEY_NOT_PLACED = 2 };   // not placed: the table is full, or may_claim() declined a new key
+template <typename Same, typename MayClaim>
+static __device__ __forceinline__ int key_table_add(unsigned long long* tags, unsigned long long* cnt, uint64_t mask, uint64_t hash, uint64_t rep, uint64_t c, Same same, MayClaim may_claim) {
+    const unsigned long long tag = (hash & 0xFFFFFFFF00000000ull) | (rep + 1);
+    uint64_t s = hash & mask;
+    for (uint64_t p = 0; p <= mask; p++, s = (s + 1) & mask) {
+        unsigned long long cur = *(volatile unsigned long long*)&tags[s];
+        if (cur == 0) {
+            if (!may_claim()) return KEY_NOT_PLACED;
+            cur = atomicCAS(&tags[s], 0ull, tag);
+            if (cur == 0) { atomicAdd(&cnt[s], (unsigned long long)c); return KEY_CLAIMED; }
+        }
+        if ((cur >> 32) != (hash >> 32)) continue;
+        if (same((cur & 0xFFFFFFFFull) - 1)) { atomicAdd(&cnt[s], (unsigned long long)c); return KEY_FOUND; }
+    }
+    return KEY_NOT_PLACED;
+}
+// Runs of equal keys (key, sub) among the lanes of a warp, in lane order: a lane without `valid` is in no run, and `merge` false puts every lane
+// in a run of its own.  Returns the run's length at its last lane (the run's head is lane - length + 1), 0 at every other lane.
+static __device__ __forceinline__ uint32_t warp_run_end(bool valid, bool merge, uint64_t key, uint32_t sub) {
+    const uint32_t lane = lane_id();
+    const uint64_t pk = __shfl_up_sync(0xffffffffu, key, 1);
+    const uint32_t ps = __shfl_up_sync(0xffffffffu, sub, 1);
+    const int pv = __shfl_up_sync(0xffffffffu, (int)valid, 1);
+    const int same_prev = merge && lane > 0 && valid && pv && pk == key && ps == sub;
+    const uint32_t heads = __ballot_sync(0xffffffffu, valid && !same_prev);
+    const int same_next = __shfl_down_sync(0xffffffffu, same_prev, 1);
+    if (!valid || (lane < 31 && same_next)) return 0;
+    const uint32_t head = 31 - __clz(heads & (0xffffffffu >> (31 - lane)));
+    return lane - head + 1;
+}
 static __device__ uint64_t hits_key_hash(const BatchView& B, const HitsQuery& q, int64_t bucket, uint32_t b, uint32_t r, unsigned long long* stats) {
     uint64_t h = mix64((uint64_t)bucket);
     uint8_t buf[VL_FMT_F64_MAX];
     for (uint32_t f = 0; f < q.nby; f++) {
-        const uint8_t* src;
-        const uint32_t len = value_text(B, q.slot[f], b, r, q.row_off8[f], buf, &src, stats);
+        const uint8_t* src; uint32_t len;
+        report_error(stats, cell_text(B, cell_at(B, q.slot[f], b), b, r, q.row_off8[f], buf, &src, &len));
         h = (h ^ len) * 0x100000001B3ull;
         for (uint32_t k = 0; k < len; k++) h = (h ^ src[k]) * 0x100000001B3ull;
         h = mix64(h);
@@ -1632,8 +1653,8 @@ static __device__ uint64_t hits_key_hash(const BatchView& B, const HitsQuery& q,
 static __device__ bool hits_same_texts(const BatchView& B, const HitsQuery& q, uint32_t b1, uint32_t r1, uint32_t b2, uint32_t r2, unsigned long long* stats) {
     uint8_t buf1[VL_FMT_F64_MAX], buf2[VL_FMT_F64_MAX];
     for (uint32_t f = 0; f < q.nby; f++) {
-        const uint8_t *s1, *s2;
-        const uint32_t l1 = value_text(B, q.slot[f], b1, r1, q.row_off8[f], buf1, &s1, stats), l2 = value_text(B, q.slot[f], b2, r2, q.row_off8[f], buf2, &s2, stats);
+        const uint8_t *s1, *s2; uint32_t l1, l2;
+        report_error(stats, max(cell_text(B, cell_at(B, q.slot[f], b1), b1, r1, q.row_off8[f], buf1, &s1, &l1), cell_text(B, cell_at(B, q.slot[f], b2), b2, r2, q.row_off8[f], buf2, &s2, &l2)));
         if (l1 != l2) return false;
         for (uint32_t k = 0; k < l1; k++) if (s1[k] != s2[k]) return false;
     }
@@ -1644,29 +1665,16 @@ static __device__ void hits_insert(const BatchView& B, const HitsQuery& q, const
                                    unsigned long long* stats) {
     if (*(volatile unsigned long long*)&T.state[1]) return;
     const uint64_t hash = hits_key_hash(B, q, bucket, b, r, stats);
-    const unsigned long long tag = (hash & 0xFFFFFFFF00000000ull) | (hit + 1);
-    uint64_t slot = hash & T.mask;
-    for (uint64_t probe = 0; probe <= T.mask; probe++, slot = (slot + 1) & T.mask) {
-        unsigned long long cur = *(volatile unsigned long long*)&T.tags[slot];
-        if (cur == 0) {
-            cur = atomicCAS(&T.tags[slot], 0ull, tag);
-            if (cur == 0) {
-                if (atomicAdd(&T.state[0], 1ull) >= T.limit) atomicExch(&T.state[1], 1ull);
-                atomicAdd(&T.cnt[slot], (unsigned long long)c);
-                return;
-            }
-        }
-        if ((cur >> 32) != (hash >> 32)) continue;
-        const uint64_t rep = (cur & 0xFFFFFFFFull) - 1;
+    const int got = key_table_add(T.tags, T.cnt, T.mask, hash, hit, c, [&](uint64_t rep) {
         const uint32_t rb = V.hit_block[rep], rr = V.hits[rep];
-        if (hit_bucket(B, q, V, rb, rr) == bucket && hits_same_texts(B, q, b, r, rb, rr, stats)) { atomicAdd(&T.cnt[slot], (unsigned long long)c); return; }
-    }
-    atomicExch(&T.state[1], 1ull);
+        return hit_bucket(B, q, V, rb, rr) == bucket && hits_same_texts(B, q, b, r, rb, rr, stats);
+    }, [] { return true; });
+    if (got == KEY_NOT_PLACED || (got == KEY_CLAIMED && atomicAdd(&T.state[0], 1ull) >= T.limit)) atomicExch(&T.state[1], 1ull);
 }
-// One CTA per block with hits.  When every by-field of the block is a dict, const or absent column its key is a function of (bucket, dict ids):
-// a single-bucket block counts its rows per dict-id code in shared memory and inserts one representative per code (with no by-fields: one
-// insert of the block's count); a multi-bucket block merges runs of equal (bucket, code) inside each warp first.  Strings and typed columns
-// insert row by row.
+// One CTA per block with hits.  When every by-field of the block is a const or absent column, or a dict cell in the plain layout
+// (plain_dict_ids), its key is a function of (bucket, dict ids): a single-bucket block counts its rows per dict-id code in shared memory and
+// inserts one representative per code (with no by-fields: one insert of the block's count); a multi-bucket block merges runs of equal
+// (bucket, code) inside each warp first.  Other cells (strings, typed, dict cells in any other layout) insert row by row.
 static __global__ void __launch_bounds__(256) k_hits_group(BatchView B, HitsQuery q, HitsView V, HitsTable T, const uint32_t* __restrict__ counts, const uint64_t* __restrict__ hit_offs,
                                                             unsigned long long* __restrict__ stats) {
     __shared__ uint32_t s_cnt[VL_HITS_CODES], s_rep[VL_HITS_CODES];
@@ -1682,10 +1690,9 @@ static __global__ void __launch_bounds__(256) k_hits_group(BatchView B, HitsQuer
             if (q.slot[f] < 0) continue;
             const DevColumn& c = B.cols[(uint64_t)b * B.nfields + q.slot[f]];
             if (c.kind != COL_VALUES) continue;
-            if (c.vt != VT_DICT) { agg = false; continue; }
             const uint32_t width = c.dict_len ? c.dict_len : 1;
-            if (codes * width > VL_HITS_CODES) { agg = false; continue; }
-            ids[f] = B.arena + c.data_off;
+            ids[f] = plain_dict_ids(B, c, B.blk_rows[b]);   // code_of reads ids only while agg holds
+            if (!ids[f] || codes * width > VL_HITS_CODES) { agg = false; continue; }
             codes *= width;
         }
         auto code_of = [&](uint32_t r) { uint32_t k = 0; for (uint32_t f = 0; f < q.nby; f++) if (ids[f]) k += ids[f][r] * stride[f]; return k; };
@@ -1705,24 +1712,14 @@ static __global__ void __launch_bounds__(256) k_hits_group(BatchView B, HitsQuer
             __syncthreads();
             continue;
         }
-        const uint32_t lane = lane_id();
         for (uint32_t base = 0; base < n; base += blockDim.x) {
             const uint32_t i = base + threadIdx.x;
-            const int valid = i < n;
+            const bool valid = i < n;
             const uint32_t r = valid ? V.hits[h0 + i] : 0;
             const int64_t bucket = valid ? hit_bucket(B, q, V, b, r) : 0;
             const uint32_t k = valid && agg ? code_of(r) : 0;
-            const int64_t pb = __shfl_up_sync(0xffffffffu, bucket, 1);
-            const uint32_t pk = __shfl_up_sync(0xffffffffu, k, 1);
-            const int pv = __shfl_up_sync(0xffffffffu, valid, 1);
-            const int same_prev = agg && lane > 0 && valid && pv && pb == bucket && pk == k;
-            const uint32_t heads = __ballot_sync(0xffffffffu, valid && !same_prev);
-            int same_next = __shfl_down_sync(0xffffffffu, same_prev, 1);
-            if (lane == 31) same_next = 0;
-            if (valid && !same_next) {
-                const uint32_t head = 31 - __clz(heads & (0xffffffffu >> (31 - lane)));
-                hits_insert(B, q, V, T, bucket, h0 + i, b, r, lane - head + 1, stats);
-            }
+            const uint32_t run = warp_run_end(valid, agg, (uint64_t)bucket, k);
+            if (run) hits_insert(B, q, V, T, bucket, h0 + i, b, r, run, stats);
         }
     }
 }
@@ -1959,10 +1956,11 @@ static __device__ __forceinline__ int facet_row_key(const BatchView& B, const Fa
     if (F.slot < 0) return FR_SKIP;
     const DevColumn& c = B.cols[(uint64_t)b * B.nfields + F.slot];
     const uint8_t* src; uint32_t len;
-    if (!cell_bytes(B, c, b, r, F.row_off8, &src, &len, stats)) {
+    const uint32_t err = cell_text_raw(B, &c, b, r, F.row_off8, &src, &len);
+    report_error(stats, err);
+    if (!err && cell_typed(&c)) {
         if (c.vt == VT_UINT8 || c.vt == VT_UINT16 || c.vt == VT_UINT32 || c.vt == VT_UINT64 || c.vt == VT_INT64) {
-            const uint32_t w = width_of_vt(c.vt);
-            const uint64_t raw = load_fixed_be(B.arena + c.data_off + (uint64_t)r * w, w);
+            const uint64_t raw = load_fixed_be(src, len);
             if (c.vt != VT_INT64) {
                 facet_num_key(k, FK_U64, raw);
                 return A.max_len <= 20 && facet_u64_len(raw) > A.max_len ? FR_DROP : FR_OK;
@@ -1988,37 +1986,14 @@ static __device__ __forceinline__ bool facet_same_key(const BatchView& B, const 
     for (uint32_t i = 0; i < k.len; i++) if (o.src[i] != k.src[i]) return false;
     return true;
 }
-// count c rows of key k (representative: hit `rep` = row r of block b) in the table tags / cnt of mask + 1 slots.  The per-field table (dropped !=
-// NULL) drops the field when it claims key number `limit` + 1 or finds no slot; a CTA's table (dropped == NULL) declines a new key once `limit` keys
-// are in it and returns false.
-static __device__ __forceinline__ bool facet_add(const BatchView& B, const FacetsArgs& A, const FacetField& F, unsigned long long* tags, unsigned long long* cnt, uint64_t mask,
-                                 unsigned long long* nkeys, uint64_t limit, unsigned int* dropped, const FKey& k, uint64_t rep, uint64_t c,
-                                 unsigned long long* __restrict__ stats) {
-    const unsigned long long tag = (k.hash & 0xFFFFFFFF00000000ull) | (rep + 1);
-    uint64_t s = k.hash & mask;
-    for (uint64_t p = 0; p <= mask; p++, s = (s + 1) & mask) {
-        unsigned long long cur = *(volatile unsigned long long*)&tags[s];
-        if (cur == 0) {
-            if (!dropped && *(volatile unsigned long long*)nkeys >= limit) return false;
-            cur = atomicCAS(&tags[s], 0ull, tag);
-            if (cur == 0) {
-                if (atomicAdd(nkeys, 1ull) >= limit && dropped) atomicExch(dropped, 1u);
-                atomicAdd(&cnt[s], (unsigned long long)c);
-                return true;
-            }
-        }
-        if ((cur >> 32) != (k.hash >> 32)) continue;
-        const uint64_t rh = (cur & 0xFFFFFFFFull) - 1;
-        if (facet_same_key(B, A, F, k, rh, stats)) { atomicAdd(&cnt[s], (unsigned long long)c); return true; }
-    }
-    if (!dropped) return false;
-    atomicExch(dropped, 1u);
-    return true;
-}
+// count c rows of key k (representative: hit `rep`) in the table of field f, which drops the field when it claims key number max_values + 1 or
+// finds no slot
 static __device__ __forceinline__ void facet_add_global(const BatchView& B, const FacetsArgs& A, const FacetField& F, uint32_t f, const FKey& k, uint64_t rep, uint64_t c,
                                                         unsigned long long* __restrict__ stats) {
     if (*(volatile unsigned int*)&A.dropped[f]) return;
-    facet_add(B, A, F, A.tags + (uint64_t)f * A.cap, A.cnt + (uint64_t)f * A.cap, A.cap - 1, &A.nkeys[f], A.max_values, &A.dropped[f], k, rep, c, stats);
+    const int got = key_table_add(A.tags + (uint64_t)f * A.cap, A.cnt + (uint64_t)f * A.cap, A.cap - 1, k.hash, rep, c,
+                                  [&](uint64_t rh) { return facet_same_key(B, A, F, k, rh, stats); }, [] { return true; });
+    if (got == KEY_NOT_PLACED || (got == KEY_CLAIMED && atomicAdd(&A.nkeys[f], 1ull) >= A.max_values)) atomicExch(&A.dropped[f], 1u);
 }
 
 // Blocks with hits whose timestamps are not all equal (minimum != maximum): the decode list of the `_time` facet.  Flat blocks are one key each.
@@ -2069,10 +2044,10 @@ static __global__ void __launch_bounds__(256) k_facets(BatchView B, FacetsArgs A
             }
             continue;
         }
-        if (!F.is_time && c->vt == VT_DICT) {
+        const uint8_t* ids = F.is_time ? nullptr : plain_dict_ids(B, *c, B.blk_rows[b]);
+        if (ids) {
             if (threadIdx.x < 8) { s_dcnt[threadIdx.x] = 0; s_drep[threadIdx.x] = 0xFFFFFFFFu; }
             __syncthreads();
-            const uint8_t* ids = B.arena + c->data_off;
             for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
                 const uint32_t id = ids[A.hits[h0 + i]];
                 if (id >= c->dict_len || id >= 8) { atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_DICT_INDEX); continue; }
@@ -2088,7 +2063,6 @@ static __global__ void __launch_bounds__(256) k_facets(BatchView B, FacetsArgs A
             continue;
         }
         if (F.is_time) {   // non-decreasing in practice: runs of equal timestamps become one insert
-            const uint32_t lane = lane_id();
             for (uint32_t base = 0; base < n; base += blockDim.x) {
                 if (base) {
                     __syncthreads();
@@ -2101,18 +2075,9 @@ static __global__ void __launch_bounds__(256) k_facets(BatchView B, FacetsArgs A
                 int fr = FR_SKIP;
                 if (valid) fr = facet_row_key(B, A, F, b, A.hits[h0 + i], h0 + i, k, stats);
                 if (fr == FR_DROP) atomicExch(&A.dropped[f], 1u);
-                const int ok = fr == FR_OK;
-                const uint64_t key = ok ? k.num : 0;
-                const uint64_t pk = __shfl_up_sync(0xffffffffu, key, 1);
-                const int pok = __shfl_up_sync(0xffffffffu, ok, 1);
-                const int same_prev = lane > 0 && ok && pok && pk == key;
-                const uint32_t heads = __ballot_sync(0xffffffffu, ok && !same_prev);
-                int same_next = __shfl_down_sync(0xffffffffu, same_prev, 1);
-                if (lane == 31) same_next = 0;
-                if (ok && !same_next) {
-                    const uint32_t head = 31 - __clz(heads & (0xffffffffu >> (31 - lane)));
-                    facet_add_global(B, A, F, f, k, h0 + i - (lane - head), lane - head + 1, stats);
-                }
+                const bool ok = fr == FR_OK;
+                const uint32_t run = warp_run_end(ok, true, ok ? k.num : 0, 0);
+                if (run) facet_add_global(B, A, F, f, k, h0 + i - (run - 1), run, stats);
             }
             continue;
         }
@@ -2129,8 +2094,12 @@ static __global__ void __launch_bounds__(256) k_facets(BatchView B, FacetsArgs A
             if (i >= n) continue;
             const int fr = facet_row_key(B, A, F, b, A.hits[h0 + i], h0 + i, k, stats);
             if (fr == FR_DROP) { atomicExch(&A.dropped[f], 1u); s_stop = 1; }
-            else if (fr == FR_OK && !facet_add(B, A, F, s_tag, s_cnt, VL_FACET_SLOTS - 1, &s_used, VL_FACET_SLOTS / 2, nullptr, k, h0 + i, 1, stats))
-                facet_add_global(B, A, F, f, k, h0 + i, 1, stats);
+            else if (fr == FR_OK) {   // the CTA table declines a new key once it is half full; such keys go to the field's table at once
+                const int got = key_table_add(s_tag, s_cnt, VL_FACET_SLOTS - 1, k.hash, h0 + i, 1, [&](uint64_t rh) { return facet_same_key(B, A, F, k, rh, stats); },
+                                              [&] { return *(volatile unsigned long long*)&s_used < VL_FACET_SLOTS / 2; });
+                if (got == KEY_CLAIMED) atomicAdd(&s_used, 1ull);
+                else if (got == KEY_NOT_PLACED) facet_add_global(B, A, F, f, k, h0 + i, 1, stats);
+            }
         }
         __syncthreads();
         if (s_stop) continue;
