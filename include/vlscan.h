@@ -345,6 +345,26 @@ typedef struct vlscan_hits_query {
 } vlscan_hits_query;
 int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_buckets, uint64_t* out_counts, uint64_t cap_groups, uint8_t* out_key_bytes,
                       uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t out_info[4]);
+/* ---- `stats by (_time:step offset off, f1, ...) count(), sum(v1), avg(v1), ...` over the selected rows of the last scan --------------------------
+ * The grouping of vlscan_hits_stats (same query, same preconditions, same groups in the same order with the same keys and row counts) plus, per
+ * group g and value field f, the partial state a stats shard exports for sum(f) and avg(f) (lib/logstorage/stats_sum.go, stats_avg.go):
+ *   out_value_counts[g * nvalues + f]: how many numbers the field gave (statsAvgProcessor.count);
+ *   out_sums[g * nvalues + f]: their sum, NaN when the count is 0 (statsSumProcessor.sum; avg's sum is the same number with 0 for NaN).
+ * The numbers of a block come from blockResultColumn.sumValues when every selected row of the block has one group key, else from
+ * getFloatValueAtRow row by row (pipe_stats.go:552-626, 700-730).  The two differ: sumValues parses strings and dict entries with tryParseNumber
+ * (durations, byte sizes: "1KiB", "5s") and counts every row of a float64 column, getFloatValueAtRow parses them with tryParseFloat64 and skips
+ * NaN float64 rows.  Both parse a const value with tryParseFloat64, read uint8..uint64 / int64 as float64(v), and take nothing from ipv4 /
+ * iso8601 columns, `_time` or a field a block lacks.
+ * A sum is the exact sum of the numbers (each cut to 92 bits below the largest of its group), rounded once: integer inputs whose sum stays below
+ * 2^53 give it exactly, and the result does not depend on the order of rows or blocks.  A group with both +Inf and -Inf, or a NaN number, sums
+ * to NaN (the reference's float adds there depend on row order).
+ *   value_names: canonical names ("" = _msg), 1 ..VLSCAN_STATS_MAX_VALUES of them; a name ending in `*` (a prefix filter such as `sum(foo*)`) is rejected.  On a
+ *   kept batch the values of every value field must have been staged in every block with selected rows (the error names the field).
+ * The caller merges batches per group key: rows and counts add, sums add with NaN as "none" (victorialogs_b200.scan.stats_merge). */
+#define VLSCAN_STATS_MAX_VALUES 4
+int vlscan_hits_sums(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* const* value_names, const size_t* value_name_lens, uint32_t nvalues, int64_t* out_buckets,
+                     uint64_t* out_counts, double* out_sums, uint64_t* out_value_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes,
+                     uint64_t* out_key_offsets, uint64_t out_info[4]);
 /* The bucket of one timestamp: host build of the routine the hits kernels run per row (truncateTimestamp above).  For tests. */
 int64_t vlscan_truncate_timestamp(int64_t ts, int64_t step, int64_t offset, uint32_t calendar);
 /* ---- the N newest selected rows: `/select/logsql/query?limit=N` (app/vlselect/logsql/logsql.go:932-948, 1005-1080 getLastNQueryResults) ---------

@@ -5,6 +5,8 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <cmath>
+#include <limits>
 #include <thread>
 #include <cstdio>
 #include <cstdlib>
@@ -778,7 +780,7 @@ void vlscan_ctx_free(vlscan_ctx* ctx) {
     for (auto& r : ctx->row_off8) r.release();
     for (auto& r : ctx->ready) r.release();
     ctx->zsrc.release(); ctx->zcols.release(); ctx->ztest.release(); ctx->ts_vals.release();
-    for (DevBuf* b : {&ctx->hit_block, &ctx->glens, &ctx->goffs, &ctx->gtiles, &ctx->gout, &ctx->gstat, &ctx->hblk, &ctx->htab, &ctx->hgrp, &ctx->lcand, &ctx->ftab, &ctx->patch, &ctx->unstaged}) b->release();
+    for (DevBuf* b : {&ctx->hit_block, &ctx->glens, &ctx->goffs, &ctx->gtiles, &ctx->gout, &ctx->gstat, &ctx->hslot, &ctx->hblk, &ctx->htab, &ctx->hgrp, &ctx->lcand, &ctx->ftab, &ctx->patch, &ctx->unstaged}) b->release();
     for (DevBuf& b : ctx->ftxt) b.release();
     zstd_dev_free(ctx->zdev);
     delete ctx->pool;
@@ -1384,17 +1386,36 @@ int vlscan_gather_values(vlscan_ctx* ctx, const char* field, size_t field_len, u
 static_assert(VLSCAN_HITS_MAX_BY == VL_HITS_MAX_BY, "the ABI's and the kernels' by-field limits differ");
 int64_t vlscan_truncate_timestamp(int64_t ts, int64_t step, int64_t offset, uint32_t calendar) { return vl::truncate_timestamp(ts, step, offset, calendar); }
 
-int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_buckets, uint64_t* out_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes,
-                      uint64_t* out_key_offsets, uint64_t out_info[4]) {
+static_assert(VLSCAN_STATS_MAX_VALUES == VL_STATS_MAX_VALUES, "the ABI's and the kernels' value-field limits differ");
+// the finished sum of one (group, value field) from its digit sums, frame and flags (k_stats_values): NaN without numbers, as newStatsProcessor
+// starts it; the exact digit total rounded once otherwise
+static double stats_sum(const int64_t d[3], int frame, unsigned flags, uint64_t count) {
+    if (!count) return std::numeric_limits<double>::quiet_NaN();
+    if ((flags & 4) || (flags & 3) == 3) return std::numeric_limits<double>::quiet_NaN();
+    if (flags & 1) return std::numeric_limits<double>::infinity();
+    if (flags & 2) return -std::numeric_limits<double>::infinity();
+    if (!frame) return 0.0;
+    const __int128 t = ((__int128)d[0] << 62) + ((__int128)d[1] << 31) + (__int128)d[2];
+    return std::ldexp((double)t, frame - VL_STATS_FRAME_BIAS - 92);
+}
+
+// vlscan_hits_stats (nv == 0) and vlscan_hits_sums: one grouping, then the value sums over the same groups
+static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* const* value_names, const size_t* value_name_lens, uint32_t nv, const char* what,
+                       int64_t* out_buckets, uint64_t* out_counts, double* out_sums, uint64_t* out_value_counts, uint64_t cap_groups, uint8_t* out_key_bytes,
+                       uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t out_info[4]) {
     uint64_t info[4] = {0, 0, 0, 0};   // groups, key bytes, selected rows, blocks whose timestamps were decoded
     const int rc = guarded(ctx, [&] {
         if (!q) throw BadInput("no hits query");
         if (q->calendar > VLSCAN_BUCKET_YEAR) throw BadInput("unknown calendar bucket kind");
         if (q->nby > VLSCAN_HITS_MAX_BY) throw BadInput("too many by-fields for the hits aggregation (at most VLSCAN_HITS_MAX_BY = 4)");
-        const std::vector<std::string> names = canonical_names(q->by_names, q->by_name_lens, q->nby, "vlscan_hits_stats");
+        const std::vector<std::string> names = canonical_names(q->by_names, q->by_name_lens, q->nby, what);
         for (const std::string& n : names)
             if (n == "_time") throw BadInput("`_time` cannot be a by-field of the hits aggregation: it is the bucket");
-        if (!ctx) throw BadInput("vlscan_hits_stats needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
+        if (nv > VLSCAN_STATS_MAX_VALUES) throw BadInput("too many value fields for vlscan_hits_sums (at most VLSCAN_STATS_MAX_VALUES = 4)");
+        const std::vector<std::string> vnames = canonical_names(value_names, value_name_lens, nv, what);
+        for (const std::string& v : vnames)
+            if (v.back() == '*') throw BadInput("value field `" + v + "`: a prefix filter such as sum(foo*) is not supported by vlscan_hits_sums");
+        if (!ctx) throw BadInput(std::string(what) + " needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
         const uint64_t n = build_hit_list(ctx, nullptr);
         if (n >= 0xFFFFFFFFull) throw BadInput("more than 2^32 - 2 selected rows in one batch");
         info[2] = n;
@@ -1406,6 +1427,13 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
         memset(&hq, 0, sizeof hq);
         hq.step = q->step; hq.offset = q->offset; hq.calendar = q->calendar; hq.nby = q->nby;
         for (uint32_t f = 0; f < q->nby; f++) { hq.slot[f] = field_slot(b, names[f]); hq.row_off8[f] = hit_row_offsets(ctx, hq.slot[f], names[f]); }
+        StatsQuery sq;
+        memset(&sq, 0, sizeof sq);
+        sq.nv = nv;
+        for (uint32_t f = 0; f < nv; f++) {   // `_time` is the bucket; its value adds nothing (isTime in sumValues / getFloatValueAtRow)
+            sq.slot[f] = vnames[f] == "_time" ? -1 : field_slot(b, vnames[f]);
+            sq.row_off8[f] = hit_row_offsets(ctx, sq.slot[f], vnames[f]);
+        }
         // buckets of the blocks; timestamps decoded only where a block spans several buckets
         unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
         uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* row_blocks = ctx->row_blocks.as<uint32_t>();
@@ -1421,12 +1449,16 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
         uint64_t max_cap = 1024; while (max_cap < 2 * n) max_cap <<= 1;
         uint64_t cap = std::min<uint64_t>(max_cap, 1 << 14);
         HitsTable T;
+        T.hit_slot = nullptr; T.slot_group = nullptr;
+        if (nv) { ctx->hslot.ensure(n * 4); T.hit_slot = ctx->hslot.as<uint32_t>(); }
         unsigned long long state[3];
+        const unsigned grid = (unsigned)std::min<uint64_t>(b->nblocks, (uint64_t)ctx->sm_count * 8);
         for (;;) {
             const size_t bytes = Carve().take(T.tags, cap).take(T.cnt, cap).take(T.state, 4).place(ctx->htab);
             T.mask = cap - 1; T.limit = cap == max_cap ? cap : cap / 2;
             VL_CUDA(cudaMemsetAsync(T.tags, 0, bytes, ctx->stream));
-            k_hits_group<<<(unsigned)std::min<uint64_t>(b->nblocks, (uint64_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(B, hq, V, T, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat);
+            if (nv) k_hits_group<true><<<grid, 256, 0, ctx->stream>>>(B, hq, V, T, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat);
+            else k_hits_group<false><<<grid, 256, 0, ctx->stream>>>(B, hq, V, T, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat);
             launch_check(ctx);
             VL_CUDA(cudaMemcpyAsync(state, T.state, sizeof state, cudaMemcpyDeviceToHost, ctx->stream));
             VL_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1439,8 +1471,23 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
         info[0] = G; info[3] = decoded;
         // the groups, then the texts of their representatives only
         long long* buckets; unsigned long long* counts; uint32_t* rep_rows; uint32_t* rep_blocks;
-        Carve().take(buckets, G).take(counts, G).take(rep_rows, G).take(rep_blocks, G).place(ctx->hgrp);
+        StatsAcc A;
+        Carve cv;
+        cv.take(buckets, G).take(counts, G).take(rep_rows, G).take(rep_blocks, G);
+        if (nv) cv.take(T.slot_group, cap).take(A.digits, 3 * G * nv).take(A.count, G * nv).take(A.frame, G * nv).take(A.flags, G * nv);
+        cv.place(ctx->hgrp);
+        if (nv) VL_CUDA(cudaMemsetAsync(A.digits, 0, (uint8_t*)(A.flags + G * nv) - (uint8_t*)A.digits, ctx->stream));
         k_hits_emit<<<cdiv(cap, 256), 256, 0, ctx->stream>>>(B, hq, V, T, rep_rows, rep_blocks, buckets, counts); launch_check(ctx);
+        std::vector<int64_t> hd(3 * G * nv); std::vector<uint64_t> hn(G * nv); std::vector<int> hf(G * nv); std::vector<unsigned> hfl(G * nv);
+        if (nv) {   // the value sums: pass 0 counts and frames, pass 1 digits (k_stats_values)
+            k_stats_values<0><<<grid, 256, 0, ctx->stream>>>(B, sq, V, T.hit_slot, T.slot_group, A, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat); launch_check(ctx);
+            k_stats_values<1><<<grid, 256, 0, ctx->stream>>>(B, sq, V, T.hit_slot, T.slot_group, A, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat); launch_check(ctx);
+            VL_CUDA(cudaMemcpyAsync(hd.data(), A.digits, hd.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(hn.data(), A.count, hn.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(hf.data(), A.frame, hf.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(hfl.data(), A.flags, hfl.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            check_gather_errors(ctx);
+        }
         std::vector<int64_t> hb(G); std::vector<uint64_t> hc(G);
         VL_CUDA(cudaMemcpyAsync(hb.data(), buckets, G * 8, cudaMemcpyDeviceToHost, ctx->stream));
         VL_CUDA(cudaMemcpyAsync(hc.data(), counts, G * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1454,7 +1501,8 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
         info[1] = key_bytes;
         if (G > cap_groups) throw BadInput("hits groups buffer too small (the needed size is reported)");
         if (key_bytes > cap_key_bytes) throw BadInput("hits key bytes buffer too small (the needed size is reported)");
-        if (!out_buckets || !out_counts || (q->nby && (!out_key_offsets || (key_bytes && !out_key_bytes)))) throw BadInput("hits output buffer missing");
+        if (!out_buckets || !out_counts || (q->nby && (!out_key_offsets || (key_bytes && !out_key_bytes))) || (nv && (!out_sums || !out_value_counts)))
+            throw BadInput("hits output buffer missing");
         // sorted by bucket, then by the key texts bytewise
         std::vector<uint64_t> order(G);
         for (uint64_t g = 0; g < G; g++) order[g] = g;
@@ -1465,10 +1513,32 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
             return false;
         });
         for (uint64_t i = 0; i < G; i++) { out_buckets[i] = hb[order[i]]; out_counts[i] = hc[order[i]]; }
+        for (uint64_t i = 0; i < G; i++)
+            for (uint32_t f = 0; f < nv; f++) {
+                const uint64_t k = order[i] * nv + f;
+                out_sums[i * nv + f] = stats_sum(&hd[3 * k], hf[k], hfl[k], hn[k]);
+                out_value_counts[i * nv + f] = hn[k];
+            }
         pack_texts(order, toffs, tbytes, out_key_bytes, out_key_offsets);
     });
     if (out_info) memcpy(out_info, info, sizeof info);
     return rc;
+}
+
+int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_buckets, uint64_t* out_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes,
+                      uint64_t* out_key_offsets, uint64_t out_info[4]) {
+    return hits_groups(ctx, q, nullptr, nullptr, 0, "vlscan_hits_stats", out_buckets, out_counts, nullptr, nullptr, cap_groups, out_key_bytes, cap_key_bytes, out_key_offsets, out_info);
+}
+
+int vlscan_hits_sums(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* const* value_names, const size_t* value_name_lens, uint32_t nvalues, int64_t* out_buckets,
+                     uint64_t* out_counts, double* out_sums, uint64_t* out_value_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes,
+                     uint64_t* out_key_offsets, uint64_t out_info[4]) {
+    if (nvalues == 0) {   // a query without value fields is vlscan_hits_stats
+        if (out_info) memset(out_info, 0, 4 * sizeof(uint64_t));
+        return guarded(ctx, [] { throw BadInput("vlscan_hits_sums: no value fields (vlscan_hits_stats counts without them)"); });
+    }
+    return hits_groups(ctx, q, value_names, value_name_lens, nvalues, "vlscan_hits_sums", out_buckets, out_counts, out_sums, out_value_counts, cap_groups, out_key_bytes,
+                       cap_key_bytes, out_key_offsets, out_info);
 }
 
 // the limit-th largest of the n int64 keys (weights: NULL = 1 each) into the radix state st (RS_COUNT words + VL_RADIX_PASSES histograms), on

@@ -1586,6 +1586,8 @@ struct HitsTable {
     unsigned long long* cnt;     // [mask + 1]
     unsigned long long* state;   // [0] slots claimed, [1] overflow, [2] groups emitted
     uint64_t mask, limit;
+    uint32_t* hit_slot;          // k_hits_group<true>: the slot of every hit (vlscan_hits_sums)
+    uint32_t* slot_group;        // [mask + 1], k_hits_emit: the group index of every occupied slot, or NULL
 };
 
 // Blocks with hits: the buckets of their minimum and maximum timestamps.  Where they are equal every row of the block is in that bucket (the
@@ -1606,10 +1608,11 @@ static __device__ __forceinline__ uint64_t mix64(uint64_t z) { z ^= z >> 30; z *
 // The key tables of the hits and the facets: open addressing, a slot holds a count and a 64-bit tag, the high half of the key's hash and 1 + the
 // index of a representative hit (0: empty).  key_table_add adds c to the slot of the key of hit `rep`: a slot whose hash half matches holds the
 // key only when same(its representative) says so, so a hash collision costs a probe, never a wrong count; an empty slot is claimed by CAS when
-// may_claim() allows it.  The caller's policy acts on the outcome.
+// may_claim() allows it.  The caller's policy acts on the outcome; *at (when given) receives the slot of a found or claimed key.
 enum { KEY_FOUND = 0, KEY_CLAIMED = 1, KEY_NOT_PLACED = 2 };   // not placed: the table is full, or may_claim() declined a new key
 template <typename Same, typename MayClaim>
-static __device__ __forceinline__ int key_table_add(unsigned long long* tags, unsigned long long* cnt, uint64_t mask, uint64_t hash, uint64_t rep, uint64_t c, Same same, MayClaim may_claim) {
+static __device__ __forceinline__ int key_table_add(unsigned long long* tags, unsigned long long* cnt, uint64_t mask, uint64_t hash, uint64_t rep, uint64_t c, Same same, MayClaim may_claim,
+                                                     uint64_t* at = nullptr) {
     const unsigned long long tag = (hash & 0xFFFFFFFF00000000ull) | (rep + 1);
     uint64_t s = hash & mask;
     for (uint64_t p = 0; p <= mask; p++, s = (s + 1) & mask) {
@@ -1617,10 +1620,10 @@ static __device__ __forceinline__ int key_table_add(unsigned long long* tags, un
         if (cur == 0) {
             if (!may_claim()) return KEY_NOT_PLACED;
             cur = atomicCAS(&tags[s], 0ull, tag);
-            if (cur == 0) { atomicAdd(&cnt[s], (unsigned long long)c); return KEY_CLAIMED; }
+            if (cur == 0) { atomicAdd(&cnt[s], (unsigned long long)c); if (at) *at = s; return KEY_CLAIMED; }
         }
         if ((cur >> 32) != (hash >> 32)) continue;
-        if (same((cur & 0xFFFFFFFFull) - 1)) { atomicAdd(&cnt[s], (unsigned long long)c); return KEY_FOUND; }
+        if (same((cur & 0xFFFFFFFFull) - 1)) { atomicAdd(&cnt[s], (unsigned long long)c); if (at) *at = s; return KEY_FOUND; }
     }
     return KEY_NOT_PLACED;
 }
@@ -1660,21 +1663,26 @@ static __device__ bool hits_same_texts(const BatchView& B, const HitsQuery& q, u
     }
     return true;
 }
-// add `c` rows with the key of hit `hit` = row r of block b, whose bucket is `bucket`
-static __device__ void hits_insert(const BatchView& B, const HitsQuery& q, const HitsView& V, const HitsTable& T, int64_t bucket, uint64_t hit, uint32_t b, uint32_t r, uint64_t c,
-                                   unsigned long long* stats) {
-    if (*(volatile unsigned long long*)&T.state[1]) return;
+// add `c` rows with the key of hit `hit` = row r of block b, whose bucket is `bucket`; returns the key's slot (meaningless once the pass overflowed:
+// the host runs it again)
+static __device__ uint32_t hits_insert(const BatchView& B, const HitsQuery& q, const HitsView& V, const HitsTable& T, int64_t bucket, uint64_t hit, uint32_t b, uint32_t r, uint64_t c,
+                                       unsigned long long* stats) {
+    if (*(volatile unsigned long long*)&T.state[1]) return 0;
     const uint64_t hash = hits_key_hash(B, q, bucket, b, r, stats);
+    uint64_t at = 0;
     const int got = key_table_add(T.tags, T.cnt, T.mask, hash, hit, c, [&](uint64_t rep) {
         const uint32_t rb = V.hit_block[rep], rr = V.hits[rep];
         return hit_bucket(B, q, V, rb, rr) == bucket && hits_same_texts(B, q, b, r, rb, rr, stats);
-    }, [] { return true; });
+    }, [] { return true; }, &at);
     if (got == KEY_NOT_PLACED || (got == KEY_CLAIMED && atomicAdd(&T.state[0], 1ull) >= T.limit)) atomicExch(&T.state[1], 1ull);
+    return (uint32_t)at;
 }
 // One CTA per block with hits.  When every by-field of the block is a const or absent column, or a dict cell in the plain layout
 // (plain_dict_ids), its key is a function of (bucket, dict ids): a single-bucket block counts its rows per dict-id code in shared memory and
 // inserts one representative per code (with no by-fields: one insert of the block's count); a multi-bucket block merges runs of equal
-// (bucket, code) inside each warp first.  Other cells (strings, typed, dict cells in any other layout) insert row by row.
+// (bucket, code) inside each warp first.  Other cells (strings, typed, dict cells in any other layout) insert row by row.  SLOTS: also write the
+// slot of every hit to T.hit_slot, for the value sums of vlscan_hits_sums (the hits-only instance compiles to the code it had without it).
+template <bool SLOTS>
 static __global__ void __launch_bounds__(256) k_hits_group(BatchView B, HitsQuery q, HitsView V, HitsTable T, const uint32_t* __restrict__ counts, const uint64_t* __restrict__ hit_offs,
                                                             unsigned long long* __restrict__ stats) {
     __shared__ uint32_t s_cnt[VL_HITS_CODES], s_rep[VL_HITS_CODES];
@@ -1698,7 +1706,14 @@ static __global__ void __launch_bounds__(256) k_hits_group(BatchView B, HitsQuer
         auto code_of = [&](uint32_t r) { uint32_t k = 0; for (uint32_t f = 0; f < q.nby; f++) if (ids[f]) k += ids[f][r] * stride[f]; return k; };
         if (agg && !V.blk_multi[b]) {
             const int64_t bucket = V.blk_bucket[b];
-            if (codes == 1) { if (threadIdx.x == 0) hits_insert(B, q, V, T, bucket, h0, b, V.hits[h0], n, stats); continue; }
+            if (codes == 1) {
+                if (!SLOTS) { if (threadIdx.x == 0) hits_insert(B, q, V, T, bucket, h0, b, V.hits[h0], n, stats); continue; }
+                if (threadIdx.x == 0) s_rep[0] = hits_insert(B, q, V, T, bucket, h0, b, V.hits[h0], n, stats);
+                __syncthreads();
+                for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) T.hit_slot[h0 + i] = s_rep[0];
+                __syncthreads();
+                continue;
+            }
             for (uint32_t k = threadIdx.x; k < codes; k += blockDim.x) { s_cnt[k] = 0; s_rep[k] = 0xFFFFFFFFu; }
             __syncthreads();
             for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
@@ -1708,8 +1723,12 @@ static __global__ void __launch_bounds__(256) k_hits_group(BatchView B, HitsQuer
             }
             __syncthreads();
             for (uint32_t k = threadIdx.x; k < codes; k += blockDim.x)
-                if (s_cnt[k]) hits_insert(B, q, V, T, bucket, h0 + s_rep[k], b, V.hits[h0 + s_rep[k]], s_cnt[k], stats);
+                if (s_cnt[k]) { const uint32_t s = hits_insert(B, q, V, T, bucket, h0 + s_rep[k], b, V.hits[h0 + s_rep[k]], s_cnt[k], stats); if (SLOTS) s_rep[k] = s; }
             __syncthreads();
+            if (SLOTS) {
+                for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) { const uint32_t k = code_of(V.hits[h0 + i]); if (k < codes) T.hit_slot[h0 + i] = s_rep[k]; }
+                __syncthreads();
+            }
             continue;
         }
         for (uint32_t base = 0; base < n; base += blockDim.x) {
@@ -1719,7 +1738,14 @@ static __global__ void __launch_bounds__(256) k_hits_group(BatchView B, HitsQuer
             const int64_t bucket = valid ? hit_bucket(B, q, V, b, r) : 0;
             const uint32_t k = valid && agg ? code_of(r) : 0;
             const uint32_t run = warp_run_end(valid, agg, (uint64_t)bucket, k);
-            if (run) hits_insert(B, q, V, T, bucket, h0 + i, b, r, run, stats);
+            uint32_t s = 0;
+            if (run) s = hits_insert(B, q, V, T, bucket, h0 + i, b, r, run, stats);
+            if (SLOTS) {   // every lane of a run takes the slot of the run's last lane
+                const uint32_t ends = __ballot_sync(0xffffffffu, run != 0);
+                const uint32_t mine = ends & (0xffffffffu << lane_id());
+                s = __shfl_sync(0xffffffffu, s, mine ? __ffs(mine) - 1 : 0);
+                if (valid) T.hit_slot[h0 + i] = s;
+            }
         }
     }
 }
@@ -1732,8 +1758,167 @@ static __global__ void k_hits_emit(BatchView B, HitsQuery q, HitsView V, HitsTab
     if (!tag) return;
     const uint64_t rep = (tag & 0xFFFFFFFFull) - 1;
     const uint64_t g = atomicAdd(&T.state[2], 1ull);
+    if (T.slot_group) T.slot_group[s] = (uint32_t)g;
     const uint32_t b = V.hit_block[rep], r = V.hits[rep];
     rep_rows[g] = r; rep_blocks[g] = b; buckets[g] = hit_bucket(B, q, V, b, r); out_counts[g] = T.cnt[s];
+}
+
+// ---- `stats by (_time:step offset off, f1, ...) sum(v...) avg(v...)`: per group and value field the sum and the count of its numbers -------------
+// (lib/logstorage/stats_sum.go, stats_avg.go; grouping pipe_stats.go:552-626, 700-730).  The reference updates a group once per block whose
+// selected rows all have its key, through blockResultColumn.sumValues (block_result.go:2501-2600), and row by row through getFloatValueAtRow
+// (:2402-2448) otherwise.  The two read a cell differently (stats_number); which one applies is decided per block from the slots of its hits
+// (k_hits_group<true>).  A sum is exact: the finite numbers of a (group, field) are added as three 31-bit integer digits in units of
+// 2^(frame - 92), frame = ilogb of the largest |number| of that (group, field), found by a first pass.  Integer adds commute, so the result does not
+// depend on the order of rows, blocks or atomics: it is the exact sum of the numbers (each cut to 2^(frame - 92), which keeps every integer below
+// 2^53 exact) rounded once on the host.  +-Inf and NaN numbers set flags instead.
+#define VL_STATS_MAX_VALUES 4
+#define VL_STATS_FRAME_BIAS 1101   // frame + bias > 0 for every finite nonzero double (ilogb >= -1074); 0 = no such number yet
+struct StatsQuery {
+    uint32_t nv;
+    int slot[VL_STATS_MAX_VALUES];                   // batch field slot of every value field; -1: no block of the batch has it (or `_time`)
+    const uint32_t* row_off8[VL_STATS_MAX_VALUES];   // k_lens_offsets of that slot
+};
+struct StatsAcc {   // per (group, value field), index g * nv + f
+    unsigned long long* digits;   // [3 * G * nv]: the digit sums, high digit first (two's complement int64)
+    unsigned long long* count;    // the numbers counted (avg's count)
+    int* frame;                   // ilogb of the largest finite nonzero |number| + VL_STATS_FRAME_BIAS, 0 = none (pass 0)
+    unsigned* flags;              // 1: a +Inf number, 2: a -Inf number, 4: a NaN number (pass 0)
+};
+struct StatsPart { long long d0, d1, d2; unsigned long long cnt; int frame; unsigned flags; };
+static __device__ __forceinline__ void stats_combine(StatsPart& a, const StatsPart& b) {
+    a.d0 += b.d0; a.d1 += b.d1; a.d2 += b.d2; a.cnt += b.cnt; a.frame = max(a.frame, b.frame); a.flags |= b.flags;
+}
+static __device__ __forceinline__ StatsPart stats_shfl_up(const StatsPart& a, uint32_t d) {
+    StatsPart o;
+    o.d0 = __shfl_up_sync(0xffffffffu, a.d0, d); o.d1 = __shfl_up_sync(0xffffffffu, a.d1, d); o.d2 = __shfl_up_sync(0xffffffffu, a.d2, d);
+    o.cnt = __shfl_up_sync(0xffffffffu, a.cnt, d); o.frame = __shfl_up_sync(0xffffffffu, a.frame, d); o.flags = __shfl_up_sync(0xffffffffu, a.flags, d);
+    return o;
+}
+static __device__ __forceinline__ StatsPart stats_shfl_xor(const StatsPart& a, uint32_t m) {
+    StatsPart o;
+    o.d0 = __shfl_xor_sync(0xffffffffu, a.d0, m); o.d1 = __shfl_xor_sync(0xffffffffu, a.d1, m); o.d2 = __shfl_xor_sync(0xffffffffu, a.d2, m);
+    o.cnt = __shfl_xor_sync(0xffffffffu, a.cnt, m); o.frame = __shfl_xor_sync(0xffffffffu, a.frame, m); o.flags = __shfl_xor_sync(0xffffffffu, a.flags, m);
+    return o;
+}
+// add `cnt` to the count and the number x (when has): pass 0 its frame or its Inf / NaN flag, pass 1 its digits relative to `frame`
+template <int PASS>
+static __device__ __forceinline__ void stats_add(StatsPart& a, double x, bool has, uint32_t cnt, int frame) {
+    a.cnt += cnt;
+    if (!has || x == 0.0) return;
+    if (isnan(x)) { a.flags |= 4; return; }
+    if (isinf(x)) { a.flags |= x > 0 ? 1 : 2; return; }
+    if (PASS == 0) { a.frame = max(a.frame, ilogb(x) + VL_STATS_FRAME_BIAS); return; }
+    // |x| < 2^(frame + 1), so |y| < 2^93; each step below subtracts the leading bits of y, which is exact
+    double y = scalbn(x, 92 - (frame - VL_STATS_FRAME_BIAS));
+    const long long d0 = (long long)scalbn(y, -62); y -= scalbn((double)d0, 62);
+    const long long d1 = (long long)scalbn(y, -31); y -= scalbn((double)d1, 31);
+    a.d0 += d0; a.d1 += d1; a.d2 += (long long)y;
+}
+template <int PASS>
+static __device__ __forceinline__ void stats_commit(const StatsAcc& A, uint64_t i, const StatsPart& a) {
+    if (PASS == 0) {
+        if (a.cnt) atomicAdd(&A.count[i], a.cnt);
+        if (a.frame) atomicMax(&A.frame[i], a.frame);
+        if (a.flags) atomicOr(&A.flags[i], a.flags);
+    } else {
+        if (a.d0) atomicAdd(&A.digits[3 * i], (unsigned long long)a.d0);
+        if (a.d1) atomicAdd(&A.digits[3 * i + 1], (unsigned long long)a.d1);
+        if (a.d2) atomicAdd(&A.digits[3 * i + 2], (unsigned long long)a.d2);
+    }
+}
+// The number of row r of a value cell (*has) and how many numbers it counts (the return value).  whole: every selected row of the block is in one
+// group (sumValues), else getFloatValueAtRow.  They differ: sumValues reads strings and dict entries with tryParseNumber (durations, byte sizes,
+// ...; a dict entry whose number is NaN is none) and counts every row of a float64 cell, NaN or not; getFloatValueAtRow reads them with
+// tryParseFloat64 and counts a float64 row only when it is not NaN.  Both read a const value with tryParseFloat64 (sumValues counts it
+// rows times: k_stats_values handles that case), integers as float64(v), and nothing from ipv4 / iso8601 cells or a field the block lacks.
+static __device__ __forceinline__ uint32_t stats_number(const BatchView& B, const DevColumn* c, uint32_t b, uint32_t r, const uint32_t* __restrict__ ro, bool whole, double* x,
+                                                        bool* has, unsigned long long* stats) {
+    *has = false;
+    if (!c || (c->kind != COL_CONST && c->kind != COL_VALUES)) return 0;
+    const uint8_t* p; uint32_t n;
+    const uint32_t err = cell_text_raw(B, c, b, r, ro, &p, &n);
+    if (err) { report_error(stats, err); return 0; }
+    const vl::mn::Span sp{p, n};
+    if (c->kind == COL_CONST || c->vt == VT_STRING || c->vt == VT_DICT) {
+        if (c->kind == COL_VALUES && whole) *has = vl::mn::parse_number(sp, x) && !(c->vt == VT_DICT && isnan(*x));
+        else *has = vl::mn::parse_f64_internal(sp, false, x);
+        return *has;
+    }
+    const uint64_t raw = load_fixed_be(p, n);
+    switch (c->vt) {
+    case VT_UINT8: case VT_UINT16: case VT_UINT32: case VT_UINT64: *x = (double)raw; *has = true; return 1;
+    case VT_INT64: *x = (double)unzigzag64(raw); *has = true; return 1;
+    case VT_FLOAT64: *x = __longlong_as_double((long long)raw); *has = !isnan(*x); return whole || *has;
+    }
+    return 0;
+}
+// One CTA per block with hits (grid-stride), each value field in turn.  A block whose hits all have one slot is one group: its numbers are
+// reduced over the CTA and committed once (a const cell: tryParseFloat64(v) * rows, counted rows times, as sumValues does).  Other blocks reduce
+// runs of equal groups inside each warp and commit once per run.  PASS 0 finds the counts, frames and flags; PASS 1 adds the digits.
+// Two launches per call, so the reference's order of float adds is not reproduced; the bound that leaves is in DESIGN §3.13.
+template <int PASS>
+static __global__ void __launch_bounds__(256) k_stats_values(BatchView B, StatsQuery sq, HitsView V, const uint32_t* __restrict__ hit_slot, const uint32_t* __restrict__ slot_group,
+                                                             StatsAcc A, const uint32_t* __restrict__ counts, const uint64_t* __restrict__ hit_offs, unsigned long long* __restrict__ stats) {
+    __shared__ StatsPart s_warp[8];
+    for (uint32_t b = blockIdx.x; b < B.nblocks; b += gridDim.x) {
+        const uint32_t n = counts[b];
+        if (n == 0) continue;
+        const uint64_t h0 = hit_offs[b];
+        const uint32_t s0 = hit_slot[h0];
+        bool same = true;
+        for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) same = same && hit_slot[h0 + i] == s0;
+        const bool whole = __syncthreads_and(same);
+        const uint32_t g0 = slot_group[s0];
+        for (uint32_t f = 0; f < sq.nv; f++) {
+            const DevColumn* c = cell_at(B, sq.slot[f], b);
+            if (whole) {
+                const int frame = PASS ? A.frame[(uint64_t)g0 * sq.nv + f] : 0;
+                StatsPart a{0, 0, 0, 0, 0, 0};
+                double x; bool has;
+                if (c && c->kind == COL_CONST) {
+                    if (threadIdx.x == 0 && stats_number(B, c, b, V.hits[h0], sq.row_off8[f], false, &x, &has, stats)) stats_add<PASS>(a, x * (double)n, true, n, frame);
+                } else {
+                    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+                        const uint32_t k = stats_number(B, c, b, V.hits[h0 + i], sq.row_off8[f], true, &x, &has, stats);
+                        stats_add<PASS>(a, x, has, k, frame);
+                    }
+                }
+#pragma unroll
+                for (uint32_t m = 16; m; m >>= 1) stats_combine(a, stats_shfl_xor(a, m));
+                if (lane_id() == 0) s_warp[threadIdx.x >> 5] = a;
+                __syncthreads();
+                if (threadIdx.x == 0) {
+                    for (uint32_t w = 1; w < (blockDim.x >> 5); w++) stats_combine(a, s_warp[w]);
+                    stats_commit<PASS>(A, (uint64_t)g0 * sq.nv + f, a);
+                }
+                __syncthreads();
+                continue;
+            }
+            for (uint32_t base = 0; base < n; base += blockDim.x) {
+                const uint32_t i = base + threadIdx.x;
+                const bool valid = i < n;
+                const uint32_t g = valid ? slot_group[hit_slot[h0 + i]] : 0xFFFFFFFFu;
+                StatsPart a{0, 0, 0, 0, 0, 0};
+                if (valid) {
+                    double x; bool has;
+                    const uint32_t k = stats_number(B, c, b, V.hits[h0 + i], sq.row_off8[f], false, &x, &has, stats);
+                    stats_add<PASS>(a, x, has, k, PASS ? A.frame[(uint64_t)g * sq.nv + f] : 0);
+                }
+                // segmented inclusive scan over runs of equal g in lane order; the last lane of a run holds its total
+                const uint32_t lane = lane_id();
+                const uint32_t gp = __shfl_up_sync(0xffffffffu, g, 1);
+                bool head = lane == 0 || gp != g;
+#pragma unroll
+                for (uint32_t d = 1; d < 32; d <<= 1) {
+                    const StatsPart o = stats_shfl_up(a, d);
+                    const bool oh = __shfl_up_sync(0xffffffffu, head, d);
+                    if (lane >= d && !head) { stats_combine(a, o); head = oh; }
+                }
+                const uint32_t gn = __shfl_down_sync(0xffffffffu, g, 1);
+                if (valid && (lane == 31 || gn != g)) stats_commit<PASS>(A, (uint64_t)g * sq.nv + f, a);
+            }
+        }
+    }
 }
 
 // ---- the N newest selected rows: `/select/logsql/query?limit=N` (app/vlselect/logsql/logsql.go:1005-1080 getLastNQueryResults) ----------------

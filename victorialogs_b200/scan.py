@@ -15,6 +15,7 @@ argument meaning as the Go structs:
 There is no CPU fallback: loading fails loudly when libvlscan.so is missing and every scan fails without a CUDA device.
 """
 import ctypes as C
+import math
 import os
 
 import numpy as np
@@ -103,7 +104,7 @@ EXPORTS = ["vlscan_device_count", "vlscan_ctx_create", "vlscan_ctx_free", "vlsca
            "vlscan_batch_upload", "vlscan_batch_free", "vlscan_batch_nblocks", "vlscan_batch_rows", "vlscan_batch_words", "vlscan_batch_device_bytes",
            "vlscan_batch_generate", "vlscan_batch_download", "vlscan_host_blocks_get", "vlscan_host_blocks_field", "vlscan_host_blocks_bytes",
            "vlscan_host_blocks_free", "vlscan_host_blocks_compress", "vlscan_zstd_decompress", "vlscan_zstd_inspect", "vlscan_zstd_walk_digest", "vlscan_part_open", "vlscan_part_free", "vlscan_part_header", "vlscan_part_nblocks", "vlscan_part_block_header", "vlscan_part_timestamps",
-           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_truncate_timestamp", "vlscan_last_rows", "vlscan_facets", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch",
+           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_hits_sums", "vlscan_truncate_timestamp", "vlscan_last_rows", "vlscan_facets", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch",
            "vlscan_scan_batch_keep", "vlscan_stage_selected"]
 
 
@@ -248,6 +249,25 @@ def facets_merge(states, limit=10, keep_const_fields=False, max_values_per_field
             continue
         ents = sorted(m.items(), key=lambda kv: (-kv[1], kv[0][1], kv[0][0]))[:limit]
         out.extend((field, text, hits) for (cls, text), hits in ents)
+    return out
+
+
+def stats_merge(states):
+    """The merge a caller runs over the per-batch states of Ctx.hits_sums (pipeStatsGroup.mergeState with statsSumProcessor.mergeState and
+    statsAvgProcessor.mergeState, lib/logstorage/stats_sum.go, stats_avg.go) -> {(bucket, key texts): (rows, [(sum, count) per value field])}.
+
+    states: lists of (bucket, keys, rows, [(sum, count)...]) as Ctx.hits_sums returns them.  Rows and counts add; a sum adds to another unless
+    one of them is NaN (a group without numbers in that batch), which takes the other.  sum(f) of a group is then its sum (NaN: no numbers),
+    avg(f) is sum / count (NaN when count is 0)."""
+    out = {}
+    for st in states:
+        for bucket, keys, rows, vals in st:
+            k = (bucket, keys)
+            if k not in out:
+                out[k] = (rows, list(vals))
+                continue
+            r0, v0 = out[k]
+            out[k] = (r0 + rows, [(b if math.isnan(a) else a if math.isnan(b) else a + b, ca + cb) for (a, ca), (b, cb) in zip(v0, vals)])
     return out
 
 
@@ -859,6 +879,36 @@ class Ctx:
             info.update(groups=out_info[0], key_bytes=out_info[1], rows=out_info[2], blocks_decoded=out_info[3])
         keys = _row_texts(kb.tobytes(), offs, int(out_info[0]), nby)
         return [(int(buckets[g]), keys[g], int(counts[g])) for g in range(int(out_info[0]))]
+
+    def hits_sums(self, step, offset=0, calendar=BUCKET_PLAIN, by=(), values=(), batch=None, info=None):
+        """`stats by (_time:step offset off, by...) count(), sum(v), avg(v)...` over the selected rows of the last scan (vlscan_hits_sums)
+        -> [(bucket, (key texts as bytes...), rows, [(sum, count) per value field])] in the order of hits_stats.  A sum is NaN when its count
+        is 0.  `info` as for hits_stats."""
+        batch = batch or getattr(self, "_last", None)
+        q, keep = hits_query(step, offset, calendar, by)
+        vn = [_b(f) for f in values]
+        varr = (C.c_char_p * max(len(vn), 1))(*vn)
+        vlens = (C.c_size_t * max(len(vn), 1))(*[len(x) for x in vn])
+        nby, nv = len(by), len(vn)
+        out_info = (C.c_uint64 * 4)()
+
+        def call(cap_groups, cap_bytes):
+            buckets = np.zeros(cap_groups, dtype=np.int64)
+            counts = np.zeros(cap_groups, dtype=np.uint64)
+            sums = np.zeros(max(cap_groups * nv, 1), dtype=np.float64)
+            vcounts = np.zeros(max(cap_groups * nv, 1), dtype=np.uint64)
+            offs = np.zeros(cap_groups * nby + 1, dtype=np.uint64)
+            kb = np.zeros(max(cap_bytes, 1), dtype=np.uint8)
+            rc = lib().vlscan_hits_sums(self.h, C.byref(q), varr, vlens, C.c_uint32(nv), buckets.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p),
+                                        sums.ctypes.data_as(C.c_void_p), vcounts.ctypes.data_as(C.c_void_p), C.c_uint64(cap_groups),
+                                        kb.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes), offs.ctypes.data_as(C.c_void_p), out_info)
+            return rc, (buckets, counts, sums, vcounts, offs, kb)
+        buckets, counts, sums, vcounts, offs, kb = self._call_grown(call, (max(1, min(int(batch.rows) if batch else 0, 1 << 16)), 1 << 16), lambda: out_info[:2])
+        if info is not None:
+            info.update(groups=out_info[0], key_bytes=out_info[1], rows=out_info[2], blocks_decoded=out_info[3])
+        G = int(out_info[0])
+        keys = _row_texts(kb.tobytes(), offs, G, nby)
+        return [(int(buckets[g]), keys[g], int(counts[g]), [(float(sums[g * nv + f]), int(vcounts[g * nv + f])) for f in range(nv)]) for g in range(G)]
 
     def last_rows(self, limit, fields=(), min_timestamp=None, info=None):
         """The `limit` newest selected rows of the last scan with _time >= min_timestamp (vlscan_last_rows)
