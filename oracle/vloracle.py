@@ -30,6 +30,20 @@ def build():
     subprocess.check_call([os.path.join(_HERE, "build.sh")], stdout=subprocess.DEVNULL)
 
 
+# the C++ restatements of the facets and stats pipes over this oracle's headers (test infrastructure next to the tests that bind them)
+COMPANIONS = (("facets_oracle", "liboracle_facets.so"), ("stats_oracle", "liboracle_stats.so"))
+
+
+def build_companions():
+    """build the restatements a tree lacks (a test directory restored without its build products), as lib() builds liboracle.so; a
+    read-only tree is left as it is"""
+    tests = os.path.join(os.path.dirname(_HERE), "tests")
+    for sub, so in COMPANIONS:
+        script = os.path.join(tests, sub, "build.sh")
+        if os.path.exists(script) and not os.path.exists(os.path.join(tests, sub, so)) and os.access(os.path.dirname(script), os.W_OK):
+            subprocess.check_call([script], stdout=subprocess.DEVNULL)
+
+
 def lib():
     global _LIB
     if _LIB is None:
@@ -40,6 +54,7 @@ def lib():
             path = os.path.join(_HERE, "liboracle.so")
         if not os.path.exists(path):
             build()
+        build_companions()
         L = C.CDLL(path)
         L.vlo_last_error.restype = C.c_char_p
         L.vlo_xxh64.restype = C.c_uint64

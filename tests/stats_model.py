@@ -4,7 +4,8 @@ goes through blockResultColumn.sumValues (block_result.go:2501-2600), any other 
 Float adds happen in the reference's order: rows in order inside a block, blocks in order.
 
 A block is {"ts": [int ns per row], "rows": [selected row indices, ascending], "cols": {name: (kind, payload)}} with kind "const" (payload: the
-value) or one of KINDS (payload: the text of every row, as the block stores it).  Parsers: the oracle's tryParseFloat64 and tryParseNumber
+value) or one of KINDS (payload: the text of every row, as the block stores it; a float64 row may instead be the double the cell holds, for
+values such as NaN, +-Inf or subnormals that no text of the writer's reaches).  Parsers: the oracle's tryParseFloat64 and tryParseNumber
 (oracle/vlo_mathnum.h, through tests/vlostats.py); the engine's own parser is not used here.
 """
 import math
@@ -23,6 +24,11 @@ def _f64(s):
 def _num(s):
     import vlostats
     return vlostats.try_parse_number(s)
+
+
+def _cell_f64(v):
+    """a float64 row: its text through tryParseFloat64, or the double itself"""
+    return v if isinstance(v, float) else _f64(v)[0]
 
 
 def sum_values(kind, payload, rows):
@@ -48,7 +54,7 @@ def sum_values(kind, payload, rows):
         return s, n
     if kind == "float64":
         for v in vals:
-            f = _f64(v)[0]
+            f = _cell_f64(v)
             if not math.isnan(f):
                 s += f
         return s, n
@@ -65,7 +71,7 @@ def value_at_row(kind, payload, r):
     if kind in ("uint8", "uint16", "uint32", "uint64", "int64"):
         return float(int(v)), True
     if kind == "float64":
-        f = _f64(v)[0]
+        f = _cell_f64(v)
         return f, not math.isnan(f)
     return 0.0, False
 
@@ -126,11 +132,13 @@ def stats(blocks, bucket_of, by, values):
 
 def close(got, want, absum, ints):
     """the device's sum against the model's: equal when every number is an integer and the total stays below 2^53, else within
-    2^-40 * sum |x| (the two add in different orders); NaN on both sides when there were no numbers"""
+    2^-40 * sum |x| (the two add in different orders); NaN on both sides when there were no numbers; a zero has the model's sign"""
     if math.isnan(want) or math.isnan(got):
         return math.isnan(want) and math.isnan(got)
     if math.isinf(want) or math.isinf(got):
         return want == got
+    if got == 0.0 and want == 0.0:
+        return math.copysign(1.0, got) == math.copysign(1.0, want)
     if ints and absum < 2.0 ** 53:
         return got == want
     return abs(got - want) <= 2.0 ** -40 * absum

@@ -1,7 +1,8 @@
 """GPU parity for `stats by (_time:step offset off, f1, ...) count(), sum(v...), avg(v...)` (vlscan_hits_sums) against the Python restatement
 (tests/stats_model.py) and the C++ one over the oracle's value decode (tests/stats_oracle via tests/vlostats.py), over the oracle's blocks, selected rows and timestamps: every column kind as a value field, all six timestamp marshal
 types, 0-3 by-fields and 1-4 value fields, plain, month and year buckets.  Groups, rows and counts are exact; a sum is exact when its numbers
-are integers adding up to less than 2^53, else within 2^-40 * sum |x|."""
+are integers adding up to less than 2^53, else within 2^-40 * sum |x|, and a zero has the restatements' sign.  The device's exactness contract
+itself is checked against exact rational sums in tests/test_gpu_zzzzzzzzzzz_stats_exact.py."""
 import math
 import random
 

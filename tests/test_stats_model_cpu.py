@@ -3,6 +3,9 @@ goes through tryParseFloat64 and counts once per row, strings and dict entries g
 (sumValues) and through tryParseFloat64 row by row otherwise, uint8..uint32 add as uint64, a float64 NaN counts in sumValues only, and a
 group without numbers sums to NaN.  Also the cross-batch merge of the per-batch states."""
 import math
+import sys
+
+import pytest
 
 import stats_model as sm
 
@@ -73,6 +76,52 @@ def test_close_bounds():
     assert sm.close(3.0, 3.0, 3.0, True) and not sm.close(3.0 + 2 ** -40, 3.0, 3.0, True)
     assert sm.close(0.1 + 0.2, 0.3, 0.5, False) and not sm.close(0.31, 0.3, 0.5, False)
     assert sm.close(math.nan, math.nan, 0.0, True) and not sm.close(0.0, math.nan, 0.0, True)
+    assert sm.close(-0.0, -0.0, 0.0, True) and not sm.close(0.0, -0.0, 0.0, True) and not sm.close(-0.0, 0.0, 0.0, False)
+
+
+def test_signed_zero_sums(oracle):
+    """the reference's sum is -0 only when every term it adds is -0: a row-path "-0" and a const "-0" (f * rows) stay -0, sumValues' total
+    over strings starts at +0"""
+    g = one({"v": ("string", [b"-0", b"x"])}, n=2, keys=[b"a", b"b"])[(0, (b"a",))]
+    assert math.copysign(1.0, g.sums[0]) < 0 and g.sums[0] == 0.0 and g.counts == [1]
+    g = one({"v": ("const", b"-0")})[(0, ())]
+    assert math.copysign(1.0, g.sums[0]) < 0 and g.counts == [4]
+    g = one({"v": ("string", [b"-0", b"-0", b"x", b"y"])})[(0, ())]
+    assert math.copysign(1.0, g.sums[0]) > 0 and g.counts == [2]
+
+
+def test_exact_sum_reference():
+    """the exact reference of tests/test_gpu_zzzzzzzzzzz_stats_exact.py on hand-computed cases"""
+    import test_gpu_zzzzzzzzzzz_stats_exact as sx
+
+    def terms(*xs):
+        t = sx.Terms()
+        t.count = len(xs)
+        for x in xs:
+            t.add(x)
+        return t
+
+    tiny, big = 2.0 ** -1074, sys.float_info.max
+    assert sx.exact(terms(2.0 ** 53, 1.0)) == 2.0 ** 53                       # the tie 2^53 + 1 goes to the even 2^53
+    assert sx.exact(terms(2.0 ** 53, 1.0, 2.0)) == 2.0 ** 53 + 4               # 2^53 + 3 rounds up
+    assert sx.exact(terms(2.0 ** 60, 1.0, -(2.0 ** 60))) == 1.0
+    assert sx.exact(terms(tiny, tiny, tiny)) == 3 * tiny                        # subnormal totals are exact
+    assert sx.exact(terms(2.0 ** -1023, 2.0 ** -1023)) == 2.0 ** -1022
+    assert sx.exact(terms(2.0 ** -1022, -tiny)) == 2.0 ** -1022 - tiny
+    assert sx.exact(terms(big, big)) == math.inf and sx.exact(terms(-big, -big)) == -math.inf
+    assert sx.exact(terms(big, 2.0 ** 970)) == math.inf                        # 2^1024 - 2^970: the tie goes to the even 2^1024
+    assert sx.exact(terms(big, 2.0 ** 969)) == big
+    assert sx.exact(terms(big, big, -big)) == big
+    for xs, sign in (((-0.0,), -1), ((-0.0, -0.0), -1), ((-0.0, 0.0), 1), ((1.0, -1.0), 1)):
+        assert math.copysign(1.0, sx.exact(terms(*xs))) == sign, xs
+    assert math.isnan(sx.exact(terms(math.inf, -math.inf))) and math.isnan(sx.exact(sx.Terms()))
+    assert sx.check_sum(2.0 ** 53, terms(2.0 ** 53, 1.0)) == "exact"
+    assert sx.check_sum(0.0, terms(2.0 ** 93, 1.0, -(2.0 ** 93))) == "bound"    # 1 is below the unit 2^(93 - 92)
+    with pytest.raises(AssertionError):
+        sx.check_sum(2.0 ** 53 + 2, terms(2.0 ** 53, 1.0))
+    with pytest.raises(AssertionError):
+        sx.check_sum(-0.0, terms(-0.0, 0.0))
+    assert sx.order_free(terms(1.0, 2.0, -0.5)) and not sx.order_free(terms(2.0 ** 60, 1.0))
 
 
 def test_stats_merge():

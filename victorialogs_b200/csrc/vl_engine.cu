@@ -1388,13 +1388,13 @@ int64_t vlscan_truncate_timestamp(int64_t ts, int64_t step, int64_t offset, uint
 
 static_assert(VLSCAN_STATS_MAX_VALUES == VL_STATS_MAX_VALUES, "the ABI's and the kernels' value-field limits differ");
 // the finished sum of one (group, value field) from its digit sums, frame and flags (k_stats_values): NaN without numbers, as newStatsProcessor
-// starts it; the exact digit total rounded once otherwise
+// starts it; the exact digit total rounded once otherwise; -0 when every term was -0 (no flag 8), as the reference's float adds give it
 static double stats_sum(const int64_t d[3], int frame, unsigned flags, uint64_t count) {
     if (!count) return std::numeric_limits<double>::quiet_NaN();
     if ((flags & 4) || (flags & 3) == 3) return std::numeric_limits<double>::quiet_NaN();
     if (flags & 1) return std::numeric_limits<double>::infinity();
     if (flags & 2) return -std::numeric_limits<double>::infinity();
-    if (!frame) return 0.0;
+    if (!frame) return (flags & 8) ? 0.0 : -0.0;
     const __int128 t = ((__int128)d[0] << 62) + ((__int128)d[1] << 31) + (__int128)d[2];
     return std::ldexp((double)t, frame - VL_STATS_FRAME_BIAS - 92);
 }

@@ -1782,7 +1782,7 @@ struct StatsAcc {   // per (group, value field), index g * nv + f
     unsigned long long* digits;   // [3 * G * nv]: the digit sums, high digit first (two's complement int64)
     unsigned long long* count;    // the numbers counted (avg's count)
     int* frame;                   // ilogb of the largest finite nonzero |number| + VL_STATS_FRAME_BIAS, 0 = none (pass 0)
-    unsigned* flags;              // 1: a +Inf number, 2: a -Inf number, 4: a NaN number (pass 0)
+    unsigned* flags;              // 1: a +Inf number, 2: a -Inf number, 4: a NaN number, 8: a counted term that is not -0 (pass 0)
 };
 struct StatsPart { long long d0, d1, d2; unsigned long long cnt; int frame; unsigned flags; };
 static __device__ __forceinline__ void stats_combine(StatsPart& a, const StatsPart& b) {
@@ -1800,10 +1800,12 @@ static __device__ __forceinline__ StatsPart stats_shfl_xor(const StatsPart& a, u
     o.cnt = __shfl_xor_sync(0xffffffffu, a.cnt, m); o.frame = __shfl_xor_sync(0xffffffffu, a.frame, m); o.flags = __shfl_xor_sync(0xffffffffu, a.flags, m);
     return o;
 }
-// add `cnt` to the count and the number x (when has): pass 0 its frame or its Inf / NaN flag, pass 1 its digits relative to `frame`
+// add `cnt` to the count and the number x (when has): pass 0 its frame or its Inf / NaN flag, pass 1 its digits relative to `frame`.  The
+// reference's sum is -0 only when every term it adds is -0, so pass 0 also flags a term that is not (8)
 template <int PASS>
 static __device__ __forceinline__ void stats_add(StatsPart& a, double x, bool has, uint32_t cnt, int frame) {
     a.cnt += cnt;
+    if (PASS == 0 && has && (x != 0.0 || !signbit(x))) a.flags |= 8;
     if (!has || x == 0.0) return;
     if (isnan(x)) { a.flags |= 4; return; }
     if (isinf(x)) { a.flags |= x > 0 ? 1 : 2; return; }
@@ -1882,6 +1884,7 @@ static __global__ void __launch_bounds__(256) k_stats_values(BatchView B, StatsQ
                         const uint32_t k = stats_number(B, c, b, V.hits[h0 + i], sq.row_off8[f], true, &x, &has, stats);
                         stats_add<PASS>(a, x, has, k, frame);
                     }
+                    if (PASS == 0 && a.cnt) a.flags |= 8;   // sumValues starts its sum at +0, so a counted block adds no -0
                 }
 #pragma unroll
                 for (uint32_t m = 16; m; m >>= 1) stats_combine(a, stats_shfl_xor(a, m));
