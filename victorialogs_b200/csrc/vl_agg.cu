@@ -1,0 +1,659 @@
+// libvlscan.so: the aggregations over the last scan's result, driven from the host: the hit list and the gathers of values and timestamps
+// (vlscan_fetch_hits, vlscan_gather_*), the hits histogram and its value sums (vlscan_hits_stats, vlscan_hits_sums), the N newest rows
+// (vlscan_last_rows) and the facets (vlscan_facets).  Their kernels are in vl_agg.cuh; row offsets come from the scan's row_offsets.
+#include <algorithm>
+#include <cmath>
+#include <cstdio>
+#include <cstring>
+#include <functional>
+#include <limits>
+#include <string>
+#include <string_view>
+#include <vector>
+#include "vl_engine.h"
+#include "vl_agg.cuh"
+
+using namespace vl;
+
+namespace {
+
+// Typed arrays laid out in one scratch buffer at 16-byte alignment: take() every array, then place() grows the buffer once, sets the pointers
+// and returns the bytes laid out.
+struct Carve {
+    size_t off = 0;
+    std::vector<std::function<void(uint8_t*)>> set;
+    template <class T> Carve& take(T*& p, uint64_t n) { const size_t o = off; off += (n * sizeof(T) + 15) & ~(size_t)15; set.push_back([&p, o](uint8_t* base) { p = (T*)(base + o); }); return *this; }
+    size_t place(DevBuf& buf) { buf.ensure(std::max<size_t>(off, 16)); for (auto& f : set) f(buf.as<uint8_t>()); return off; }
+};
+
+}  // namespace
+
+extern "C" {
+
+// ---- hit materialisation ----------------------------------------------------------------------------------------------------------------------
+// hits of the last scan on the device: ctx->hits (row inside its block), ctx->hit_block, ctx->hit_offs (first hit of every block); returns their number
+static uint64_t build_hit_list(vlscan_ctx* ctx, uint64_t* out_hit_offsets) {
+    if (!ctx->has_result) throw BadInput("no scan result on this ctx");
+    VL_CUDA(cudaSetDevice(ctx->device));
+    const vlscan_batch* b = ctx->last_batch;
+    BatchView B = b->view();
+    ctx->hit_offs.ensure((b->nblocks + 1) * 8);
+    uint64_t* offs = ctx->hit_offs.as<uint64_t>();
+    k_scan_cta<uint32_t><<<1, 1024, 0, ctx->stream>>>(ctx->counts.as<uint32_t>(), (uint32_t)b->nblocks, offs, offs + b->nblocks); launch_check(ctx);
+    uint64_t total = 0;
+    VL_CUDA(cudaMemcpyAsync(&total, offs + b->nblocks, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_hit_offsets) VL_CUDA(cudaMemcpyAsync(out_hit_offsets, offs, (b->nblocks + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    VL_CUDA(cudaStreamSynchronize(ctx->stream));
+    ctx->hits.ensure(std::max<uint64_t>(total, 4) * 4); ctx->hit_block.ensure(std::max<uint64_t>(total, 4) * 4);
+    if (b->nblocks && total) {
+        k_hits_compact<<<cdiv((uint64_t)b->nblocks * 32, 256), 256, 0, ctx->stream>>>(B, ctx->regs[0].as<uint64_t>(), offs, ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), total);
+        launch_check(ctx);
+    }
+    ctx->gstat.ensure(ST_COUNT * 8);
+    VL_CUDA(cudaMemsetAsync(ctx->gstat.p, 0, ST_COUNT * 8, ctx->stream));
+    return total;
+}
+
+int vlscan_fetch_hits(vlscan_ctx* ctx, uint32_t* out_hit_rows, uint64_t cap, uint64_t* out_hit_offsets) {
+    return guarded(ctx, [&] {
+        if (!ctx->has_result) throw BadInput("no scan result to fetch on this ctx");
+        const uint64_t total = build_hit_list(ctx, out_hit_offsets);
+        if (total > cap) throw BadInput("hit buffer too small");
+        if (total) VL_CUDA(cudaMemcpyAsync(out_hit_rows, ctx->hits.p, total * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaStreamSynchronize(ctx->stream));
+    });
+}
+
+static void check_gather_errors(vlscan_ctx* ctx) {
+    unsigned long long h[ST_COUNT];
+    VL_CUDA(cudaMemcpyAsync(h, ctx->gstat.p, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
+    VL_CUDA(cudaStreamSynchronize(ctx->stream));
+    static const char* const msg[] = {"", "cannot unmarshal strings: row lengths do not add up to the data length", "too big index for dict value", "unexpected length for binary representation of a number", "", "",
+                                      "the timestamps of a block with selected rows were not handed over", "cannot unmarshal timestamps",
+                                      "the values of a cell with selected rows are not on the device (vlscan_stage_selected stages them)",
+                                      "the decoded timestamps of a block contradict the minimum / maximum of its header"};
+    if (h[ST_ERROR]) throw BadInput(msg[std::min<unsigned long long>(h[ST_ERROR], 9)]);
+}
+// the timestamps of the blocks in `list` (wc[WC_ROW] of them) decoded into ctx->ts_vals, at each block's first word * 64; errors go to gstat
+static const unsigned long long* decode_listed_timestamps(vlscan_ctx* ctx, const BatchView& B, const uint32_t* list, const uint32_t* wc) {
+    ctx->ts_vals.ensure(B.nwords * 64 * 8);
+    k_ts_decode_list<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(B, list, wc, ctx->ts_vals.as<unsigned long long>(), ctx->gstat.as<unsigned long long>()); launch_check(ctx);
+    return ctx->ts_vals.as<unsigned long long>();
+}
+
+int vlscan_gather_timestamps(vlscan_ctx* ctx, int64_t* out_timestamps, uint64_t cap, uint64_t* out_hit_offsets) {
+    return guarded(ctx, [&] {
+        const uint64_t n = build_hit_list(ctx, out_hit_offsets);
+        if (n > cap) throw BadInput("timestamps buffer too small");
+        if (!n) return;
+        const vlscan_batch* b = ctx->last_batch;
+        BatchView B = b->view();
+        uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* row_blocks = ctx->row_blocks.as<uint32_t>();
+        VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
+        k_hit_blocks_list<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), -1, 1, row_blocks, wc); launch_check(ctx);
+        const unsigned long long* ts_vals = decode_listed_timestamps(ctx, B, row_blocks, wc);
+        ctx->gout.ensure(n * 8);
+        k_gather_ts<<<cdiv(n, 256), 256, 0, ctx->stream>>>(B, ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), n, ts_vals, ctx->gout.as<long long>()); launch_check(ctx);
+        check_gather_errors(ctx);
+        VL_CUDA(cudaMemcpy(out_timestamps, ctx->gout.p, n * 8, cudaMemcpyDeviceToHost));
+    });
+}
+
+// row offsets of the blocks with hits whose cell in column `slot` has per-row lens items (cell_needs_offsets; kept from the scan where it already
+// computed them); `with_rows` (default: the scan's counts) != 0 marks the blocks whose offsets are needed.  On a kept batch every such block
+// must have the field's values on the device: the call fails naming the field otherwise (the kernels would report ERR_VALUES_ABSENT, which
+// cannot say which field it was).
+static const uint32_t* hit_row_offsets(vlscan_ctx* ctx, int slot, const std::string& name, const uint32_t* with_rows = nullptr) {
+    if (slot < 0) return nullptr;
+    BatchView B = ctx->last_batch->view();
+    if (ctx->last_batch->split_hdr && B.nblocks) {   // only a bloom-first / kept staging leaves values on the host
+        ctx->unstaged.ensure(16);
+        VL_CUDA(cudaMemsetAsync(ctx->unstaged.p, 0, 8, ctx->stream));
+        k_unstaged_count<<<cdiv(B.nblocks, 256), 256, 0, ctx->stream>>>(B, with_rows ? with_rows : ctx->counts.as<uint32_t>(), slot, ctx->unstaged.as<unsigned long long>());
+        launch_check(ctx);
+        unsigned long long n = 0;
+        VL_CUDA(cudaMemcpyAsync(&n, ctx->unstaged.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaStreamSynchronize(ctx->stream));
+        if (n) throw BadInput("field `" + name + "`: its values are not on the device in " + std::to_string(n) + " block(s) with selected rows (stage them with vlscan_stage_selected)");
+    }
+    uint32_t* wc = ctx->work_count.as<uint32_t>();
+    VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
+    k_hit_blocks_list<<<cdiv(B.nblocks, 256), 256, 0, ctx->stream>>>(B, with_rows ? with_rows : ctx->counts.as<uint32_t>(), slot, 0, ctx->lens_blocks.as<uint32_t>(), wc); launch_check(ctx);
+    return row_offsets(ctx, B, slot, ctx->lens_blocks.as<uint32_t>(), wc, ctx->gstat.as<unsigned long long>(), WC_LENS);
+}
+// exclusive scan of the n lengths into offs[0 .. n], offs[n] = the total: tile sums, their scan by one CTA, per-tile prefixes
+static void exclusive_scan(vlscan_ctx* ctx, const uint32_t* lens, uint64_t n, uint64_t* offs) {
+    const uint64_t ntiles = cdiv(n, VL_SCAN_TILE);
+    ctx->gtiles.ensure((ntiles + 1) * 8);
+    k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(lens, n, ctx->gtiles.as<unsigned long long>(), nullptr, 0); launch_check(ctx);
+    k_scan_cta<uint64_t><<<1, 1024, 0, ctx->stream>>>(ctx->gtiles.as<uint64_t>(), (uint32_t)ntiles, ctx->gtiles.as<uint64_t>(), offs + n); launch_check(ctx);
+    k_scan_tiles<<<(unsigned)ntiles, 256, 0, ctx->stream>>>(lens, n, ctx->gtiles.as<unsigned long long>(), (unsigned long long*)offs, 1); launch_check(ctx);
+}
+// texts of column `slot` in the n rows (rows[i], blocks[i]): their lengths and exclusive offsets go to ctx->glens / ctx->goffs (goffs[n] = the
+// total, also returned; synchronises), then text_bytes writes the bytes to ctx->gout
+static uint64_t text_offsets(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint32_t* rows, const uint32_t* blocks, uint64_t n) {
+    BatchView B = ctx->last_batch->view();
+    ctx->glens.ensure(n * 4); ctx->goffs.ensure((n + 1) * 8);
+    k_gather_values<<<cdiv(n, 128), 128, 0, ctx->stream>>>(B, slot, rows, blocks, n, ro, 0, ctx->glens.as<uint32_t>(), nullptr, nullptr, ctx->gstat.as<unsigned long long>()); launch_check(ctx);
+    exclusive_scan(ctx, ctx->glens.as<uint32_t>(), n, ctx->goffs.as<uint64_t>());
+    uint64_t total = 0;
+    VL_CUDA(cudaMemcpyAsync(&total, ctx->goffs.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    check_gather_errors(ctx);
+    return total;
+}
+static void text_bytes(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint32_t* rows, const uint32_t* blocks, uint64_t n, uint64_t total) {
+    ctx->gout.ensure(std::max<uint64_t>(total, 16));
+    k_gather_values<<<cdiv(n, 128), 128, 0, ctx->stream>>>(ctx->last_batch->view(), slot, rows, blocks, n, ro, 1, nullptr, ctx->goffs.as<uint64_t>(), ctx->gout.as<uint8_t>(), ctx->gstat.as<unsigned long long>());
+    launch_check(ctx);
+}
+// the texts of column `slot` in the n rows (rows[i], blocks[i]) on the host: text i is bytes[offs[i] .. offs[i + 1])
+static void host_texts(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint32_t* rows, const uint32_t* blocks, uint64_t n, std::vector<uint64_t>& offs,
+                       std::vector<uint8_t>& bytes) {
+    const uint64_t total = text_offsets(ctx, slot, ro, rows, blocks, n);
+    offs.resize(n + 1); bytes.resize(total);
+    text_bytes(ctx, slot, ro, rows, blocks, n, total);
+    VL_CUDA(cudaMemcpyAsync(offs.data(), ctx->goffs.p, (n + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (total) VL_CUDA(cudaMemcpyAsync(bytes.data(), ctx->gout.p, total, cudaMemcpyDeviceToHost, ctx->stream));
+    check_gather_errors(ctx);   // synchronises
+}
+// rows x fields output: row i is row order[i] of the per-field texts (host_texts); the text of field f in row i ends at out_offsets[i * nf + f + 1]
+static void pack_texts(const std::vector<uint64_t>& order, const std::vector<std::vector<uint64_t>>& toffs, const std::vector<std::vector<uint8_t>>& tbytes,
+                       uint8_t* out_bytes, uint64_t* out_offsets) {
+    const size_t nf = toffs.size();
+    uint64_t o = 0;
+    for (uint64_t i = 0; i < order.size(); i++)
+        for (size_t f = 0; f < nf; f++) {
+            const uint64_t a = toffs[f][order[i]], len = toffs[f][order[i] + 1] - a;
+            if (len) memcpy(out_bytes + o, tbytes[f].data() + a, len);
+            o += len;
+            out_offsets[i * nf + f + 1] = o;
+        }
+}
+
+int vlscan_gather_values(vlscan_ctx* ctx, const char* field, size_t field_len, uint8_t* out_bytes, uint64_t cap_bytes, uint64_t* out_value_offsets, uint64_t cap_values,
+                         uint64_t* out_total_bytes, uint64_t* out_hit_offsets) {
+    if (out_total_bytes) *out_total_bytes = 0;
+    return guarded(ctx, [&] {
+        const uint64_t n = build_hit_list(ctx, out_hit_offsets);
+        if (n > cap_values) throw BadInput("value offsets buffer too small");
+        if (out_value_offsets) out_value_offsets[0] = 0;
+        if (!n) return;
+        std::string name(field, field_len); if (name.empty()) name = "_msg";   // getCanonicalColumnName
+        const int slot = ctx->last_batch->field_slot(name);
+        const uint32_t* ro = hit_row_offsets(ctx, slot, name);
+        const uint32_t* rows = ctx->hits.as<uint32_t>(); const uint32_t* blocks = ctx->hit_block.as<uint32_t>();
+        const uint64_t total = text_offsets(ctx, slot, ro, rows, blocks, n);
+        if (out_total_bytes) *out_total_bytes = total;
+        if (total > cap_bytes) throw BadInput("values buffer too small (the needed size is reported)");
+        text_bytes(ctx, slot, ro, rows, blocks, n, total);
+        if (out_value_offsets) VL_CUDA(cudaMemcpyAsync(out_value_offsets, ctx->goffs.p, (n + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        if (total) VL_CUDA(cudaMemcpyAsync(out_bytes, ctx->gout.p, total, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaStreamSynchronize(ctx->stream));
+    });
+}
+
+static_assert(VLSCAN_HITS_MAX_BY == VL_HITS_MAX_BY, "the ABI's and the kernels' by-field limits differ");
+int64_t vlscan_truncate_timestamp(int64_t ts, int64_t step, int64_t offset, uint32_t calendar) { return vl::truncate_timestamp(ts, step, offset, calendar); }
+
+static_assert(VLSCAN_STATS_MAX_VALUES == VL_STATS_MAX_VALUES, "the ABI's and the kernels' value-field limits differ");
+// the finished sum of one (group, value field) from its digit sums, frame and flags (k_stats_values): NaN without numbers, as newStatsProcessor
+// starts it; the exact digit total rounded once otherwise; -0 when every term was -0 (no flag 8), as the reference's float adds give it
+static double stats_sum(const int64_t d[3], int frame, unsigned flags, uint64_t count) {
+    if (!count) return std::numeric_limits<double>::quiet_NaN();
+    if ((flags & 4) || (flags & 3) == 3) return std::numeric_limits<double>::quiet_NaN();
+    if (flags & 1) return std::numeric_limits<double>::infinity();
+    if (flags & 2) return -std::numeric_limits<double>::infinity();
+    if (!frame) return (flags & 8) ? 0.0 : -0.0;
+    const __int128 t = ((__int128)d[0] << 62) + ((__int128)d[1] << 31) + (__int128)d[2];
+    return std::ldexp((double)t, frame - VL_STATS_FRAME_BIAS - 92);
+}
+
+// vlscan_hits_stats (nv == 0) and vlscan_hits_sums: one grouping, then the value sums over the same groups
+static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* const* value_names, const size_t* value_name_lens, uint32_t nv, const char* what,
+                       int64_t* out_buckets, uint64_t* out_counts, double* out_sums, uint64_t* out_value_counts, uint64_t cap_groups, uint8_t* out_key_bytes,
+                       uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t out_info[4]) {
+    uint64_t info[4] = {0, 0, 0, 0};   // groups, key bytes, selected rows, blocks whose timestamps were decoded
+    const int rc = guarded(ctx, [&] {
+        if (!q) throw BadInput("no hits query");
+        if (q->calendar > VLSCAN_BUCKET_YEAR) throw BadInput("unknown calendar bucket kind");
+        if (q->nby > VLSCAN_HITS_MAX_BY) throw BadInput("too many by-fields for the hits aggregation (at most VLSCAN_HITS_MAX_BY = 4)");
+        const std::vector<std::string> names = canonical_names(q->by_names, q->by_name_lens, q->nby, what);
+        for (const std::string& n : names)
+            if (n == "_time") throw BadInput("`_time` cannot be a by-field of the hits aggregation: it is the bucket");
+        if (nv > VLSCAN_STATS_MAX_VALUES) throw BadInput("too many value fields for vlscan_hits_sums (at most VLSCAN_STATS_MAX_VALUES = 4)");
+        const std::vector<std::string> vnames = canonical_names(value_names, value_name_lens, nv, what);
+        for (const std::string& v : vnames)
+            if (v.back() == '*') throw BadInput("value field `" + v + "`: a prefix filter such as sum(foo*) is not supported by vlscan_hits_sums");
+        if (!ctx) throw BadInput(std::string(what) + " needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
+        const uint64_t n = build_hit_list(ctx, nullptr);
+        if (n >= 0xFFFFFFFFull) throw BadInput("more than 2^32 - 2 selected rows in one batch");
+        info[2] = n;
+        if (out_key_offsets) out_key_offsets[0] = 0;
+        if (!n) return;
+        const vlscan_batch* b = ctx->last_batch;
+        BatchView B = b->view();
+        HitsQuery hq;
+        memset(&hq, 0, sizeof hq);
+        hq.step = q->step; hq.offset = q->offset; hq.calendar = q->calendar; hq.nby = q->nby;
+        for (uint32_t f = 0; f < q->nby; f++) { hq.slot[f] = b->field_slot(names[f]); hq.row_off8[f] = hit_row_offsets(ctx, hq.slot[f], names[f]); }
+        StatsQuery sq;
+        memset(&sq, 0, sizeof sq);
+        sq.nv = nv;
+        for (uint32_t f = 0; f < nv; f++) {   // `_time` is the bucket; its value adds nothing (isTime in sumValues / getFloatValueAtRow)
+            sq.slot[f] = vnames[f] == "_time" ? -1 : b->field_slot(vnames[f]);
+            sq.row_off8[f] = hit_row_offsets(ctx, sq.slot[f], vnames[f]);
+        }
+        // buckets of the blocks; timestamps decoded only where a block spans several buckets
+        unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
+        uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* row_blocks = ctx->row_blocks.as<uint32_t>();
+        long long* blk_bucket; uint8_t* blk_multi;
+        Carve().take(blk_bucket, b->nblocks).take(blk_multi, b->nblocks).place(ctx->hblk);
+        VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
+        k_hits_classify<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), hq, blk_bucket, blk_multi, row_blocks, wc, gstat); launch_check(ctx);
+        const unsigned long long* ts_vals = decode_listed_timestamps(ctx, B, row_blocks, wc);
+        uint32_t decoded = 0;
+        VL_CUDA(cudaMemcpyAsync(&decoded, wc + WC_ROW, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        HitsView V{ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), blk_bucket, blk_multi, ts_vals};
+        // the group table: starts small, grows by 8x while a pass overflows; at 2 x the hit count it cannot overflow
+        uint64_t max_cap = 1024; while (max_cap < 2 * n) max_cap <<= 1;
+        uint64_t cap = std::min<uint64_t>(max_cap, 1 << 14);
+        HitsTable T;
+        T.hit_slot = nullptr; T.slot_group = nullptr;
+        if (nv) { ctx->hslot.ensure(n * 4); T.hit_slot = ctx->hslot.as<uint32_t>(); }
+        unsigned long long state[3];
+        const unsigned grid = (unsigned)std::min<uint64_t>(b->nblocks, (uint64_t)ctx->sm_count * 8);
+        for (;;) {
+            const size_t bytes = Carve().take(T.tags, cap).take(T.cnt, cap).take(T.state, 4).place(ctx->htab);
+            T.mask = cap - 1; T.limit = cap == max_cap ? cap : cap / 2;
+            VL_CUDA(cudaMemsetAsync(T.tags, 0, bytes, ctx->stream));
+            if (nv) k_hits_group<true><<<grid, 256, 0, ctx->stream>>>(B, hq, V, T, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat);
+            else k_hits_group<false><<<grid, 256, 0, ctx->stream>>>(B, hq, V, T, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat);
+            launch_check(ctx);
+            VL_CUDA(cudaMemcpyAsync(state, T.state, sizeof state, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaStreamSynchronize(ctx->stream));
+            if (!state[1]) break;
+            if (cap == max_cap) throw BadInput("hits aggregation: group table overflow");
+            cap = std::min(cap * 8, max_cap);
+        }
+        check_gather_errors(ctx);
+        const uint64_t G = state[0];
+        info[0] = G; info[3] = decoded;
+        // the groups, then the texts of their representatives only
+        long long* buckets; unsigned long long* counts; uint32_t* rep_rows; uint32_t* rep_blocks;
+        StatsAcc A;
+        Carve cv;
+        cv.take(buckets, G).take(counts, G).take(rep_rows, G).take(rep_blocks, G);
+        if (nv) cv.take(T.slot_group, cap).take(A.digits, 3 * G * nv).take(A.count, G * nv).take(A.frame, G * nv).take(A.flags, G * nv);
+        cv.place(ctx->hgrp);
+        if (nv) VL_CUDA(cudaMemsetAsync(A.digits, 0, (uint8_t*)(A.flags + G * nv) - (uint8_t*)A.digits, ctx->stream));
+        k_hits_emit<<<cdiv(cap, 256), 256, 0, ctx->stream>>>(B, hq, V, T, rep_rows, rep_blocks, buckets, counts); launch_check(ctx);
+        std::vector<int64_t> hd(3 * G * nv); std::vector<uint64_t> hn(G * nv); std::vector<int> hf(G * nv); std::vector<unsigned> hfl(G * nv);
+        if (nv) {   // the value sums: pass 0 counts and frames, pass 1 digits (k_stats_values)
+            k_stats_values<0><<<grid, 256, 0, ctx->stream>>>(B, sq, V, T.hit_slot, T.slot_group, A, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat); launch_check(ctx);
+            k_stats_values<1><<<grid, 256, 0, ctx->stream>>>(B, sq, V, T.hit_slot, T.slot_group, A, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat); launch_check(ctx);
+            VL_CUDA(cudaMemcpyAsync(hd.data(), A.digits, hd.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(hn.data(), A.count, hn.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(hf.data(), A.frame, hf.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(hfl.data(), A.flags, hfl.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            check_gather_errors(ctx);
+        }
+        std::vector<int64_t> hb(G); std::vector<uint64_t> hc(G);
+        VL_CUDA(cudaMemcpyAsync(hb.data(), buckets, G * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaMemcpyAsync(hc.data(), counts, G * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        std::vector<std::vector<uint64_t>> toffs(q->nby); std::vector<std::vector<uint8_t>> tbytes(q->nby);
+        uint64_t key_bytes = 0;
+        for (uint32_t f = 0; f < q->nby; f++) {
+            host_texts(ctx, hq.slot[f], hq.row_off8[f], rep_rows, rep_blocks, G, toffs[f], tbytes[f]);
+            key_bytes += tbytes[f].size();
+        }
+        VL_CUDA(cudaStreamSynchronize(ctx->stream));
+        info[1] = key_bytes;
+        if (G > cap_groups) throw BadInput("hits groups buffer too small (the needed size is reported)");
+        if (key_bytes > cap_key_bytes) throw BadInput("hits key bytes buffer too small (the needed size is reported)");
+        if (!out_buckets || !out_counts || (q->nby && (!out_key_offsets || (key_bytes && !out_key_bytes))) || (nv && (!out_sums || !out_value_counts)))
+            throw BadInput("hits output buffer missing");
+        // sorted by bucket, then by the key texts bytewise
+        std::vector<uint64_t> order(G);
+        for (uint64_t g = 0; g < G; g++) order[g] = g;
+        auto text = [&](uint32_t f, uint64_t g) { return std::string_view((const char*)tbytes[f].data() + toffs[f][g], toffs[f][g + 1] - toffs[f][g]); };
+        std::sort(order.begin(), order.end(), [&](uint64_t x, uint64_t y) {
+            if (hb[x] != hb[y]) return hb[x] < hb[y];
+            for (uint32_t f = 0; f < q->nby; f++) { const int c = text(f, x).compare(text(f, y)); if (c) return c < 0; }
+            return false;
+        });
+        for (uint64_t i = 0; i < G; i++) { out_buckets[i] = hb[order[i]]; out_counts[i] = hc[order[i]]; }
+        for (uint64_t i = 0; i < G; i++)
+            for (uint32_t f = 0; f < nv; f++) {
+                const uint64_t k = order[i] * nv + f;
+                out_sums[i * nv + f] = stats_sum(&hd[3 * k], hf[k], hfl[k], hn[k]);
+                out_value_counts[i * nv + f] = hn[k];
+            }
+        pack_texts(order, toffs, tbytes, out_key_bytes, out_key_offsets);
+    });
+    if (out_info) memcpy(out_info, info, sizeof info);
+    return rc;
+}
+
+int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_buckets, uint64_t* out_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes,
+                      uint64_t* out_key_offsets, uint64_t out_info[4]) {
+    return hits_groups(ctx, q, nullptr, nullptr, 0, "vlscan_hits_stats", out_buckets, out_counts, nullptr, nullptr, cap_groups, out_key_bytes, cap_key_bytes, out_key_offsets, out_info);
+}
+
+int vlscan_hits_sums(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* const* value_names, const size_t* value_name_lens, uint32_t nvalues, int64_t* out_buckets,
+                     uint64_t* out_counts, double* out_sums, uint64_t* out_value_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes,
+                     uint64_t* out_key_offsets, uint64_t out_info[4]) {
+    if (nvalues == 0) {   // a query without value fields is vlscan_hits_stats
+        if (out_info) memset(out_info, 0, 4 * sizeof(uint64_t));
+        return guarded(ctx, [] { throw BadInput("vlscan_hits_sums: no value fields (vlscan_hits_stats counts without them)"); });
+    }
+    return hits_groups(ctx, q, value_names, value_name_lens, nvalues, "vlscan_hits_sums", out_buckets, out_counts, out_sums, out_value_counts, cap_groups, out_key_bytes,
+                       cap_key_bytes, out_key_offsets, out_info);
+}
+
+// the limit-th largest of the n int64 keys (weights: NULL = 1 each) into the radix state st (RS_COUNT words + VL_RADIX_PASSES histograms), on
+// the stream, with no host round trip
+static void radix_select(vlscan_ctx* ctx, const long long* keys, const uint32_t* weights, uint64_t n, uint64_t limit, unsigned long long* st) {
+    VL_CUDA(cudaMemsetAsync(st, 0, (RS_COUNT + VL_RADIX_PASSES * 256) * 8, ctx->stream));
+    const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(cdiv(n, 256), (uint64_t)ctx->sm_count * 8));
+    for (int p = 0; p < VL_RADIX_PASSES; p++) {
+        const int shift = 64 - 8 * (p + 1);
+        unsigned long long* hist = st + RS_COUNT + p * 256;
+        k_radix_hist<<<grid, 256, 0, ctx->stream>>>(keys, weights, n, st, shift, hist); launch_check(ctx);
+        k_radix_pick<<<1, 32, 0, ctx->stream>>>(hist, shift, limit, st); launch_check(ctx);
+    }
+}
+
+int vlscan_last_rows(vlscan_ctx* ctx, const vlscan_last_query* q, int64_t* out_timestamps, uint32_t* out_blocks, uint32_t* out_rows, uint64_t cap_rows,
+                     uint8_t* out_bytes, uint64_t cap_bytes, uint64_t* out_offsets, uint64_t out_info[4]) {
+    uint64_t info[4] = {0, 0, 0, 0};   // rows returned, value bytes, selected rows, blocks whose timestamps were decoded
+    const int rc = guarded(ctx, [&] {
+        if (!q) throw BadInput("no last-rows query");
+        if (q->limit == 0) throw BadInput("the limit of vlscan_last_rows must be at least 1");
+        const std::vector<std::string> names = canonical_names(q->field_names, q->field_name_lens, q->nfields, "vlscan_last_rows");
+        for (const std::string& n : names)
+            if (n == "_time") throw BadInput("`_time` cannot be a field of vlscan_last_rows: it is returned in out_timestamps");
+        if (!ctx) throw BadInput("vlscan_last_rows needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
+        if (!ctx->has_result) throw BadInput("no scan result on this ctx");
+        VL_CUDA(cudaSetDevice(ctx->device));
+        const vlscan_batch* b = ctx->last_batch;
+        BatchView B = b->view();
+        const uint64_t nb = b->nblocks, limit = q->limit;
+        const long long floor_ts = q->min_timestamp;
+        const uint32_t* counts = ctx->counts.as<uint32_t>();
+        ctx->gstat.ensure(ST_COUNT * 8);
+        VL_CUDA(cudaMemsetAsync(ctx->gstat.p, 0, ST_COUNT * 8, ctx->stream));
+        unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
+        long long* blk_key; uint64_t* cand_offs; uint32_t* blk_w; uint32_t* cand_rows; uint32_t* blk_mark; uint32_t* cand; uint32_t* decode;
+        Carve().take(blk_key, nb).take(cand_offs, nb + 1).take(blk_w, nb).take(cand_rows, nb).take(blk_mark, nb).take(cand, nb).take(decode, nb).place(ctx->hblk);
+        const size_t st_words = RS_COUNT + VL_RADIX_PASSES * 256;
+        unsigned long long* st_blk; unsigned long long* st_row;
+        Carve().take(st_blk, st_words).take(st_row, st_words).place(ctx->htab);
+        ctx->hit_offs.ensure((nb + 1) * 8);
+        uint64_t* hit_offs = ctx->hit_offs.as<uint64_t>();
+        k_scan_cta<uint32_t><<<1, 1024, 0, ctx->stream>>>(counts, (uint32_t)nb, hit_offs, hit_offs + nb); launch_check(ctx);
+        // (1) the block threshold T_lo, from the headers alone
+        if (nb) { k_last_block_keys<<<cdiv(nb, 256), 256, 0, ctx->stream>>>(B, counts, floor_ts, blk_key, blk_w, gstat); launch_check(ctx); }
+        radix_select(ctx, blk_key, blk_w, nb, limit, st_blk);
+        // (2) the candidate blocks, the timestamps of those that are not flat, and the count of their selected rows >= T_lo
+        uint32_t* wc = ctx->work_count.as<uint32_t>();
+        VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
+        VL_CUDA(cudaMemsetAsync(cand_rows, 0, nb * 4, ctx->stream));
+        VL_CUDA(cudaMemsetAsync(blk_mark, 0, nb * 4, ctx->stream));
+        if (nb) { k_last_candidates<<<cdiv(nb, 256), 256, 0, ctx->stream>>>(B, counts, floor_ts, st_blk, cand, decode, wc); launch_check(ctx); }
+        const unsigned long long* ts_vals = decode_listed_timestamps(ctx, B, decode, wc);
+        const unsigned row_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(nb, (uint64_t)ctx->sm_count * 8));
+        k_last_rows<<<row_grid, 256, 0, ctx->stream>>>(B, ctx->regs[0].as<uint64_t>(), cand, wc, ts_vals, floor_ts, st_blk, 0, cand_rows, nullptr, nullptr, nullptr, nullptr, gstat);
+        launch_check(ctx);
+        k_scan_cta<uint32_t><<<1, 1024, 0, ctx->stream>>>(cand_rows, (uint32_t)nb, cand_offs, cand_offs + nb); launch_check(ctx);
+        uint64_t selected = 0, M = 0; unsigned long long blk_short = 0; uint32_t decoded = 0;
+        VL_CUDA(cudaMemcpyAsync(&selected, hit_offs + nb, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaMemcpyAsync(&M, cand_offs + nb, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaMemcpyAsync(&blk_short, st_blk + RS_SHORT, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        VL_CUDA(cudaMemcpyAsync(&decoded, wc + WC_ROW, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        check_gather_errors(ctx);   // synchronises
+        info[2] = selected; info[3] = decoded;
+        if (selected >= 0xFFFFFFFFull) throw BadInput("more than 2^32 - 2 selected rows in one batch");
+        // the block weights promise `limit` rows >= T_lo; fewer means a block's timestamps disagree with its header
+        if (!blk_short && M < limit) throw BadInput("the decoded timestamps of a block contradict the minimum / maximum of its header");
+        const uint64_t n = std::min<uint64_t>(limit, M);
+        std::vector<int64_t> hts(n); std::vector<uint32_t> hb(n), hr(n);
+        uint32_t* sel_blk = nullptr; uint32_t* sel_row = nullptr;
+        if (n) {
+            // the candidates in (block, row) order, then (3) the exact top N: T_N, every row above it and the last ties
+            long long* cts; uint32_t* cblk; uint32_t* crow;
+            Carve().take(cts, M).take(cblk, M).take(crow, M).place(ctx->lcand);
+            k_last_rows<<<row_grid, 256, 0, ctx->stream>>>(B, ctx->regs[0].as<uint64_t>(), cand, wc, ts_vals, floor_ts, st_blk, 1, nullptr, cand_offs, cts, cblk, crow, gstat);
+            launch_check(ctx);
+            radix_select(ctx, cts, nullptr, M, limit, st_row);
+            ctx->glens.ensure(M * 4); ctx->goffs.ensure((M + 1) * 8);
+            k_last_ties<<<cdiv(M, 256), 256, 0, ctx->stream>>>(cts, M, st_row, ctx->glens.as<uint32_t>()); launch_check(ctx);
+            exclusive_scan(ctx, ctx->glens.as<uint32_t>(), M, ctx->goffs.as<uint64_t>());
+            long long* sel_ts; unsigned long long* sel_n;
+            Carve().take(sel_ts, n).take(sel_n, 1).take(sel_blk, n).take(sel_row, n).place(ctx->hgrp);
+            VL_CUDA(cudaMemsetAsync(sel_n, 0, 8, ctx->stream));
+            k_last_choose<<<cdiv(M, 256), 256, 0, ctx->stream>>>(cts, cblk, crow, M, st_row, ctx->goffs.as<uint64_t>(), sel_ts, sel_blk, sel_row, sel_n, blk_mark); launch_check(ctx);
+            uint64_t chosen = 0;
+            VL_CUDA(cudaMemcpyAsync(&chosen, sel_n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(hts.data(), sel_ts, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(hb.data(), sel_blk, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(hr.data(), sel_row, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaStreamSynchronize(ctx->stream));
+            if (chosen != n) throw BadInput("internal: the top-N selection chose " + std::to_string(chosen) + " rows instead of " + std::to_string(n));
+        }
+        // (4) the texts of the chosen rows only
+        std::vector<std::vector<uint64_t>> toffs(q->nfields); std::vector<std::vector<uint8_t>> tbytes(q->nfields);
+        uint64_t value_bytes = 0;
+        for (uint32_t f = 0; f < q->nfields && n; f++) {
+            const int slot = b->field_slot(names[f]);
+            host_texts(ctx, slot, hit_row_offsets(ctx, slot, names[f], blk_mark), sel_row, sel_blk, n, toffs[f], tbytes[f]);
+            value_bytes += tbytes[f].size();
+        }
+        if (!q->nfields) check_gather_errors(ctx);   // else host_texts checked them after the last kernel
+        info[0] = n; info[1] = value_bytes;
+        if (n > cap_rows) throw BadInput("rows buffer too small (the needed size is reported)");
+        if (value_bytes > cap_bytes) throw BadInput("value bytes buffer too small (the needed size is reported)");
+        if ((n && (!out_timestamps || !out_blocks || !out_rows)) || (q->nfields && !out_offsets) || (value_bytes && !out_bytes)) throw BadInput("last-rows output buffer missing");
+        // ascending (timestamp, block, row): getLastNRows' order
+        std::vector<uint64_t> order(n);
+        for (uint64_t i = 0; i < n; i++) order[i] = i;
+        std::sort(order.begin(), order.end(), [&](uint64_t x, uint64_t y) {
+            if (hts[x] != hts[y]) return hts[x] < hts[y];
+            if (hb[x] != hb[y]) return hb[x] < hb[y];
+            return hr[x] < hr[y];
+        });
+        if (out_offsets) out_offsets[0] = 0;
+        for (uint64_t i = 0; i < n; i++) { out_timestamps[i] = hts[order[i]]; out_blocks[i] = hb[order[i]]; out_rows[i] = hr[order[i]]; }
+        pack_texts(order, toffs, tbytes, out_bytes, out_offsets);
+    });
+    if (out_info) memcpy(out_info, info, sizeof info);
+    return rc;
+}
+
+// marshalTimestampRFC3339NanoString in UTC: "2006-01-02T15:04:05" (fmt_iso8601's first 19 bytes), the fraction without its trailing zeros, "Z"
+static std::string rfc3339_nano(int64_t ts) {
+    uint8_t buf[32];
+    fmt_iso8601(buf, ts);
+    std::string s((const char*)buf, 19);
+    int64_t frac = ts % 1000000000LL;
+    if (frac < 0) frac += 1000000000LL;
+    if (frac) {
+        char f[16];
+        snprintf(f, sizeof f, ".%09lld", (long long)frac);
+        size_t n = strlen(f);
+        while (f[n - 1] == '0') n--;
+        s.append(f, n);
+    }
+    return s + "Z";
+}
+
+int vlscan_facets(vlscan_ctx* ctx, const vlscan_facets_query* q, uint8_t* out_dropped, uint64_t* out_field_offsets, uint64_t* out_hits, uint8_t* out_classes,
+                  uint64_t cap_entries, uint8_t* out_bytes, uint64_t cap_bytes, uint64_t* out_value_offsets, uint64_t out_info[4]) {
+    uint64_t info[4] = {0, 0, 0, 0};   // entries, value bytes, selected rows, blocks whose timestamps were decoded
+    const int rc = guarded(ctx, [&] {
+        if (!q) throw BadInput("no facets query");
+        if (q->nfields == 0) throw BadInput("vlscan_facets needs at least one field");
+        const std::vector<std::string> names = canonical_names(q->field_names, q->field_name_lens, q->nfields, "vlscan_facets");
+        for (auto n = names.begin(); n != names.end(); ++n) {
+            if (*n == "_stream" || *n == "_stream_id") throw BadInput("`" + *n + "` facets are not computed by the engine: it does not know the streams of the blocks");
+            if (std::find(names.begin(), n, *n) != n) throw BadInput("duplicate facets field `" + *n + "`");
+        }
+        const uint64_t max_values = q->max_values_per_field ? q->max_values_per_field : VLSCAN_FACETS_DEFAULT_MAX_VALUES;
+        const uint64_t max_len = q->max_value_len ? q->max_value_len : VLSCAN_FACETS_DEFAULT_MAX_VALUE_LEN;
+        if (!ctx) throw BadInput("vlscan_facets needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
+        const uint64_t n = build_hit_list(ctx, nullptr);
+        if (n >= 0xFFFFFFFFull) throw BadInput("more than 2^32 - 2 selected rows in one batch");
+        info[2] = n;
+        const uint32_t nf = q->nfields;
+        std::vector<uint8_t> dropped(nf, 0);
+        std::vector<uint64_t> field_off(nf + 1, 0);
+        std::vector<uint64_t> ehits, evoff(1, 0);
+        std::vector<uint8_t> ecls;
+        std::string ebytes;
+        if (n) {
+            const vlscan_batch* b = ctx->last_batch;
+            BatchView B = b->view();
+            // small device state: the field table, the entry bases and cursors, a work counter, a flag, the blocks with hits
+            FacetField* d_fields; uint64_t* d_base; unsigned long long* d_cursor; uint32_t* d_wc; unsigned int* d_flag; uint32_t* d_blocks;
+            Carve().take(d_fields, nf).take(d_base, nf + 1).take(d_cursor, nf).take(d_wc, WC_COUNT).take(d_flag, 1).take(d_blocks, b->nblocks + 1).place(ctx->hblk);
+            VL_CUDA(cudaMemsetAsync(d_wc, 0, WC_COUNT * 4, ctx->stream));
+            k_hit_blocks_list<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), -1, 1, d_blocks, d_wc); launch_check(ctx);
+            uint32_t nblk = 0;
+            VL_CUDA(cudaMemcpyAsync(&nblk, d_wc + WC_ROW, 4, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaStreamSynchronize(ctx->stream));
+            std::vector<FacetField> hf(nf);
+            bool has_time = false;
+            if (ctx->ftxt.size() < nf) ctx->ftxt.resize(nf);
+            for (uint32_t f = 0; f < nf; f++) {
+                FacetField& F = hf[f];
+                F.is_time = names[f] == "_time";
+                F.slot = F.is_time ? -1 : b->field_slot(names[f]);
+                F.row_off8 = hit_row_offsets(ctx, F.slot, names[f]);
+                F.toffs = nullptr; F.tbytes = nullptr;
+                has_time |= F.is_time;
+                if (F.slot < 0 || !nblk) continue;
+                // a field stored as float64 / ipv4 / iso8601 in a block with hits: the texts of every hit, formatted by the gather kernels first, so
+                // that no formatter runs inside the facets pass
+                unsigned int formatted = 0;
+                VL_CUDA(cudaMemsetAsync(d_flag, 0, 4, ctx->stream));
+                k_facets_formatted<<<cdiv(nblk, 256), 256, 0, ctx->stream>>>(B, d_blocks, nblk, F.slot, d_flag); launch_check(ctx);
+                VL_CUDA(cudaMemcpyAsync(&formatted, d_flag, 4, cudaMemcpyDeviceToHost, ctx->stream));
+                VL_CUDA(cudaStreamSynchronize(ctx->stream));
+                if (!formatted) continue;
+                const uint64_t total = text_offsets(ctx, F.slot, F.row_off8, ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), n);
+                text_bytes(ctx, F.slot, F.row_off8, ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), n, total);
+                DevBuf& T = ctx->ftxt[f];
+                T.ensure((n + 1) * 8 + total + 16);
+                VL_CUDA(cudaMemcpyAsync(T.p, ctx->goffs.p, (n + 1) * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+                if (total) VL_CUDA(cudaMemcpyAsync(T.as<uint8_t>() + (n + 1) * 8, ctx->gout.p, total, cudaMemcpyDeviceToDevice, ctx->stream));
+                F.toffs = T.as<uint64_t>(); F.tbytes = T.as<uint8_t>() + (n + 1) * 8;
+            }
+            // one table per field, bounded by the keys it can hold before it is dropped (saturating: max_values may be UINT64_MAX)
+            const uint64_t bound = std::min(max_values, n - 1) + 1;
+            uint64_t cap = 16;
+            while (cap < 2 * bound) cap <<= 1;
+            const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)nblk * nf, (uint64_t)ctx->sm_count * 4));
+            const uint64_t table_bytes = (uint64_t)nf * cap * 16 + nf * 16 + 64;
+            size_t free_b = 0, total_b = 0;
+            VL_CUDA(cudaMemGetInfo(&free_b, &total_b));
+            if (cap > (1ull << 40) / 16 || table_bytes > ctx->ftab.cap + free_b / 2)
+                throw BadInput("vlscan_facets: max_values_per_field = " + std::to_string(max_values) + " needs " + std::to_string(table_bytes >> 20) + " MiB of facet tables for " +
+                               std::to_string(nf) + " fields, more than the device has free");
+            ctx->ftab.ensure(table_bytes);
+            VL_CUDA(cudaMemcpyAsync(d_fields, hf.data(), nf * sizeof(FacetField), cudaMemcpyHostToDevice, ctx->stream));
+            FacetsArgs A;
+            A.fields = d_fields; A.nf = nf; A.blocks = d_blocks; A.nblocks = nblk; A.max_values = max_values; A.max_len = max_len;
+            A.hits = ctx->hits.as<uint32_t>(); A.hit_block = ctx->hit_block.as<uint32_t>(); A.hit_offs = ctx->hit_offs.as<uint64_t>(); A.counts = ctx->counts.as<uint32_t>();
+            A.tags = ctx->ftab.as<unsigned long long>(); A.cnt = A.tags + (uint64_t)nf * cap; A.nkeys = A.cnt + (uint64_t)nf * cap; A.dropped = (unsigned int*)(A.nkeys + nf);
+            A.cap = cap; A.ts_vals = nullptr;
+            VL_CUDA(cudaMemsetAsync(A.tags, 0, table_bytes, ctx->stream));
+            unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
+            uint32_t decoded = 0;
+            if (has_time) {   // timestamps of the blocks with hits that are not flat
+                uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* row_blocks = ctx->row_blocks.as<uint32_t>();
+                VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
+                k_facets_ts_list<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, A.counts, row_blocks, wc, gstat); launch_check(ctx);
+                A.ts_vals = decode_listed_timestamps(ctx, B, row_blocks, wc);
+                VL_CUDA(cudaMemcpyAsync(&decoded, wc + WC_ROW, 4, cudaMemcpyDeviceToHost, ctx->stream));
+                check_gather_errors(ctx);
+            }
+            info[3] = decoded;
+            k_facets<<<grid, 256, 0, ctx->stream>>>(B, A, gstat); launch_check(ctx);
+            std::vector<unsigned long long> nkeys(nf); std::vector<uint32_t> drop(nf);
+            VL_CUDA(cudaMemcpyAsync(nkeys.data(), A.nkeys, nf * 8, cudaMemcpyDeviceToHost, ctx->stream));
+            VL_CUDA(cudaMemcpyAsync(drop.data(), A.dropped, nf * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            check_gather_errors(ctx);   // synchronises
+            for (uint32_t f = 0; f < nf; f++) {
+                dropped[f] = drop[f] ? 1 : 0;
+                field_off[f + 1] = field_off[f] + (dropped[f] ? 0 : nkeys[f]);
+            }
+            const uint64_t E = field_off[nf];
+            std::vector<uint32_t> cls(E), rrows(E), rblocks(E); std::vector<unsigned long long> nums(E), cnts(E);
+            uint32_t* rep_rows; uint32_t* rep_blocks; uint32_t* d_cls; unsigned long long* d_nums; unsigned long long* d_cnts; uint32_t* str_rows; uint32_t* str_blocks;
+            Carve().take(rep_rows, E).take(rep_blocks, E).take(d_cls, E).take(d_nums, E).take(d_cnts, E).take(str_rows, E).take(str_blocks, E).place(ctx->hgrp);
+            if (E) {   // the entries field after field
+                VL_CUDA(cudaMemcpyAsync(d_base, field_off.data(), nf * 8, cudaMemcpyHostToDevice, ctx->stream));
+                VL_CUDA(cudaMemsetAsync(d_cursor, 0, nf * 8, ctx->stream));
+                k_facets_emit<<<grid, 256, 0, ctx->stream>>>(B, A, d_base, d_cursor, rep_rows, rep_blocks, d_cls, d_nums, d_cnts, gstat); launch_check(ctx);
+                VL_CUDA(cudaMemcpyAsync(cls.data(), d_cls, E * 4, cudaMemcpyDeviceToHost, ctx->stream));
+                VL_CUDA(cudaMemcpyAsync(nums.data(), d_nums, E * 8, cudaMemcpyDeviceToHost, ctx->stream));
+                VL_CUDA(cudaMemcpyAsync(cnts.data(), d_cnts, E * 8, cudaMemcpyDeviceToHost, ctx->stream));
+                VL_CUDA(cudaMemcpyAsync(rrows.data(), rep_rows, E * 4, cudaMemcpyDeviceToHost, ctx->stream));
+                VL_CUDA(cudaMemcpyAsync(rblocks.data(), rep_blocks, E * 4, cudaMemcpyDeviceToHost, ctx->stream));
+                check_gather_errors(ctx);
+            }
+            for (uint32_t f = 0; f < nf; f++) {
+                const uint64_t e0 = field_off[f], ne = field_off[f + 1] - e0;
+                if (!ne) continue;
+                std::vector<std::string> text(ne);
+                // the texts of the string-class representatives only
+                std::vector<uint64_t> str_of; std::vector<uint32_t> sr, sb;
+                for (uint64_t i = 0; i < ne; i++)
+                    if (cls[e0 + i] == FK_STR) { str_of.push_back(i); sr.push_back(rrows[e0 + i]); sb.push_back(rblocks[e0 + i]); }
+                if (!str_of.empty()) {
+                    const uint64_t ns = str_of.size();
+                    VL_CUDA(cudaMemcpyAsync(str_rows, sr.data(), ns * 4, cudaMemcpyHostToDevice, ctx->stream));
+                    VL_CUDA(cudaMemcpyAsync(str_blocks, sb.data(), ns * 4, cudaMemcpyHostToDevice, ctx->stream));
+                    std::vector<uint64_t> toffs; std::vector<uint8_t> tbytes;
+                    host_texts(ctx, hf[f].slot, hf[f].row_off8, str_rows, str_blocks, ns, toffs, tbytes);
+                    for (uint64_t k = 0; k < ns; k++) text[str_of[k]].assign((const char*)tbytes.data() + toffs[k], toffs[k + 1] - toffs[k]);
+                }
+                std::vector<uint8_t> ecl(ne);
+                for (uint64_t i = 0; i < ne; i++) {
+                    const uint64_t e = e0 + i;
+                    char nb[24];
+                    switch (cls[e]) {
+                    case FK_U64: snprintf(nb, sizeof nb, "%llu", (unsigned long long)nums[e]); text[i] = nb; ecl[i] = VLSCAN_FACET_UINT64; break;
+                    case FK_NEG: snprintf(nb, sizeof nb, "%lld", (long long)nums[e]); text[i] = nb; ecl[i] = VLSCAN_FACET_NEGATIVE; break;
+                    case FK_TIME: text[i] = rfc3339_nano((int64_t)nums[e]); ecl[i] = VLSCAN_FACET_STRING; break;
+                    default: ecl[i] = VLSCAN_FACET_STRING;   // its text was gathered above
+                    }
+                }
+                // hits descending, then text bytewise, then class: a total order, where the reference's sort.Slice leaves ties unordered
+                std::vector<uint64_t> order(ne);
+                for (uint64_t i = 0; i < ne; i++) order[i] = i;
+                std::sort(order.begin(), order.end(), [&](uint64_t x, uint64_t y) {
+                    if (cnts[e0 + x] != cnts[e0 + y]) return cnts[e0 + x] > cnts[e0 + y];
+                    const int c = text[x].compare(text[y]);
+                    return c ? c < 0 : ecl[x] < ecl[y];
+                });
+                for (uint64_t i : order) {
+                    ehits.push_back(cnts[e0 + i]); ecls.push_back(ecl[i]);
+                    ebytes += text[i]; evoff.push_back(ebytes.size());
+                }
+            }
+        }
+        info[0] = ehits.size(); info[1] = ebytes.size();
+        if (info[0] > cap_entries) throw BadInput("facets entries buffer too small (the needed size is reported)");
+        if (info[1] > cap_bytes) throw BadInput("facets value bytes buffer too small (the needed size is reported)");
+        if (!out_dropped || !out_field_offsets || !out_value_offsets || (info[0] && (!out_hits || !out_classes)) || (info[1] && !out_bytes)) throw BadInput("facets output buffer missing");
+        memcpy(out_dropped, dropped.data(), nf);
+        memcpy(out_field_offsets, field_off.data(), (nf + 1) * 8);
+        memcpy(out_value_offsets, evoff.data(), evoff.size() * 8);
+        if (info[0]) { memcpy(out_hits, ehits.data(), info[0] * 8); memcpy(out_classes, ecls.data(), info[0]); }
+        if (info[1]) memcpy(out_bytes, ebytes.data(), info[1]);
+    });
+    if (out_info) memcpy(out_info, info, sizeof info);
+    return rc;
+}
+
+}  // extern "C"

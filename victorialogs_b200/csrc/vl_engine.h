@@ -1,5 +1,10 @@
-// Internal structures of libvlscan.so shared by vl_engine.cu (staging, scan interpreter, C ABI) and vl_gen.cu
-// (synthetic batch generator).
+// Internal host-side structures of libvlscan.so shared by vl_engine.cu (staging, scan interpreter, C ABI), vl_agg.cu (the aggregations
+// over a scan's result), vl_gen.cu (synthetic batch generator) and vl_zstd.cu (device ZSTD decoder driver).
+//
+// This header holds no device code.  A __global__ is defined in exactly one file, and exactly one .cu includes that file: nvcc emits every
+// non-template static kernel in each translation unit that includes its definition, launched there or not, so a kernel header included
+// twice compiles and ships its kernels twice.  vl_kernels.cuh belongs to vl_engine.cu, vl_agg.cuh to vl_agg.cu; device helpers both use
+// are plain __device__ functions in vl_cell.cuh.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,7 +12,7 @@
 #include <string>
 #include <vector>
 #include "../../include/vlscan.h"
-#include "vl_kernels.cuh"
+#include "vl_types.h"
 #include "vl_zstd.h"
 #include "vl_zstd_walk.h"   // BadInput
 #include "vl_hostpool.h"
@@ -72,6 +77,11 @@ struct vlscan_batch {
     void note_columns(const std::vector<vl::DevColumn>& cols) {
         slot_vt_mask.assign(nfields, 0);
         for (size_t i = 0; i < cols.size(); i++) if (cols[i].kind == vl::COL_VALUES) slot_vt_mask[i % nfields] |= 1u << cols[i].vt;
+    }
+    // batch field slot of a canonical field name, -1 when no block of the batch has it
+    int field_slot(const std::string& name) const {
+        for (uint32_t s = 0; s < nfields; s++) if (field_names[s] == name) return (int)s;
+        return -1;
     }
     vl::BatchView view() const {
         vl::BatchView v;
@@ -146,4 +156,28 @@ struct vlscan_ctx {
 namespace vl {
 // fills word_block / init_bitmap / blk_* device arrays of a batch from host row counts (shared by upload + generate)
 void finish_batch_layout(vlscan_ctx* ctx, vlscan_batch* b, const std::vector<uint32_t>& rows);
+
+// row_off8 of column `slot` (k_lens_offsets) for the blocks in `list` (wc[wc_slot] of them) that this scan has not computed yet; ready[slot]
+// is cleared by the first call of a scan.  Returns ctx->row_off8[slot].  Errors go to stats.
+const uint32_t* row_offsets(vlscan_ctx* ctx, const BatchView& B, int slot, const uint32_t* list, const uint32_t* wc, unsigned long long* stats, int wc_slot);
+
+// ---- error plumbing --------------------------------------------------------------------------------------------------
+template <class F> int guarded(vlscan_ctx* ctx, F&& f) {
+    try { f(); return 0; }
+    catch (const CudaFail& e) { set_thread_error(e.msg); if (ctx) ctx->err = e.msg; return e.code > 0 ? e.code : 1; }
+    catch (const BadInput& e) { set_thread_error(e.msg); if (ctx) ctx->err = e.msg; return -1; }
+    catch (const ProgError& e) { set_thread_error(e.what()); if (ctx) ctx->err = e.what(); return -2; }
+    catch (const std::exception& e) { set_thread_error(e.what()); if (ctx) ctx->err = e.what(); return -3; }
 }
+
+inline void launch_check(vlscan_ctx* ctx) { ctx->launches++; VL_CUDA(cudaGetLastError()); }
+inline unsigned cdiv(uint64_t a, uint64_t b) { return (unsigned)((a + b - 1) / b); }
+
+// the canonical names of a caller's n field names ("" is `_msg`: getCanonicalColumnName)
+inline std::vector<std::string> canonical_names(const char* const* names, const size_t* lens, uint32_t n, const char* what) {
+    if (n && (!names || !lens)) throw BadInput(std::string(what) + ": field names missing");
+    std::vector<std::string> out;
+    for (uint32_t f = 0; f < n; f++) out.push_back(lens[f] ? std::string(names[f], lens[f]) : "_msg");
+    return out;
+}
+}  // namespace vl

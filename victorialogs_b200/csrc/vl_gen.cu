@@ -20,6 +20,7 @@
 #include <cstring>
 #include <vector>
 #include "vl_engine.h"
+#include "vl_hd.cuh"
 
 using namespace vl;
 

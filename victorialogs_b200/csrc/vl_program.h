@@ -19,8 +19,6 @@
 
 namespace vl {
 
-struct ProgError : std::runtime_error { using std::runtime_error::runtime_error; };
-
 // ---- host helpers -------------------------------------------------------------------------------------------------
 template <class F> inline void host_each_token(const std::string& s, F&& f) {   // tokenizer.go:34-117
     const uint8_t* p = (const uint8_t*)s.data(); uint32_t n = (uint32_t)s.size();

@@ -1,6 +1,8 @@
-// POD layouts shared by the host program compiler (vl_program.cpp) and the CUDA engine (vl_engine.cu).
+// Layouts and codes shared by the host program compiler (vl_program.h), the host side of the engine (vl_engine.h) and the kernels
+// (vl_kernels.cuh, vl_agg.cuh).  No device code.
 #pragma once
 #include <stdint.h>
+#include <stdexcept>
 
 namespace vl {
 
@@ -129,5 +131,37 @@ enum { PAIR_STRINGS = 0,   // the string forms of both values (const, missing = 
        PAIR_DICT = 2 };    // both dict columns: the dictionary entries
 // scan verifier modes of the row-agnostic substring kernel
 enum { SCAN_PHRASE = 0, SCAN_PREFIX = 1, SCAN_CONTAINS = 2, SCAN_RX_DOTPLUS = 3, SCAN_RX_SUFFIX = 4, SCAN_RX_TAIL = 5 };
+
+// the device image of a compiled program (vlscan_program::image): the tables of vl_program.h's Program
+struct DevProgram {
+    const DevLeaf* leaves; const DevPrepass* prepass; const DevRegex* regexes;
+    const uint8_t* blob; const uint64_t* u64s; const uint32_t* u32s;
+};
+
+// stats slots (device u64 array)
+enum { ST_VALUES_BYTES = 0, ST_BLOOM_BYTES, ST_COLUMNS_READ, ST_BITMAP_BYTES, ST_ROWS_MATCHED, ST_BLOCKS_MATCHED, ST_ERROR, ST_SCAN_BYTES, ST_COUNT };
+// atomicMax keeps the largest code: the numbers rank the errors (4 and 5 are unused)
+enum { ERR_NONE = 0, ERR_LENS_MISMATCH = 1, ERR_DICT_INDEX = 2, ERR_BAD_WIDTH = 3, ERR_NO_TIMESTAMPS = 6, ERR_BAD_TIMESTAMPS = 7, ERR_VALUES_ABSENT = 8,
+       ERR_TS_HEADER = 9 };   // decoded timestamps outside the [min, max] of their block header (k_last_rows)
+
+// work counters of the kernels' block and tile lists (k_plan_leaf, k_plan_pair, k_hit_blocks_list)
+enum { WC_LENS = 0, WC_TILES = 1, WC_ROW = 2, WC_LENS2 = 3, WC_COUNT = 4 };   // WC_LENS2: the second column of a two-column leaf
+
+// a resident batch as the kernels see it (vlscan_batch::view)
+struct BatchView {
+    const uint8_t* arena;         // values payloads: lens items, data, encoded timestamps (lens_off, data_off, DevTimestamps.off)
+    const uint8_t* hdr;           // header payloads: bloom filters, const values, dict tables (bloom_off, meta_off).  The same buffer as `arena`
+                                  // unless the batch was staged bloom-first (vlscan_scan_batch): then it is the phase-1 buffer
+    const DevColumn* cols;        // [nblocks * nfields]
+    const uint32_t* blk_rows;     // [nblocks]
+    const uint64_t* blk_word_off; // [nblocks + 1]
+    const uint32_t* word_block;   // [nwords] owning block of each bitmap word
+    const DevTimestamps* ts;      // [nblocks] or NULL when the batch was staged without timestamps
+    uint32_t nblocks, nfields;
+    uint64_t nwords;
+};
+
+// a filter tree the program compiler rejects (vlscan_program_create returns -2)
+struct ProgError : std::runtime_error { using std::runtime_error::runtime_error; };
 
 }  // namespace vl
