@@ -69,6 +69,28 @@ def scan_batch_both_ways(ctx, prog, hb):
     return w0, c0, s0
 
 
+def numeric_and_special_columns(n=300):
+    """one block's columns of every kind: uint8 / uint16 / uint32 / uint64 / int64, ipv4, iso8601, dict, const and a string column"""
+    return [
+        ("u8", [b"%d" % (i % 200) for i in range(n)]),
+        ("u16", [b"%d" % (i * 37 % 60000) for i in range(n)]),
+        ("u32", [b"%d" % (i * 104729 % 4000000000) for i in range(n)]),
+        ("u64", [b"%d" % (i * 1234567890123 + 5000000000) for i in range(n)]),
+        ("i64", [b"%d" % ((i - 150) * 987654321) for i in range(n)]),
+        ("ip", [b"10.%d.%d.%d" % (i % 3, i % 251, (i * 7) % 256) for i in range(n)]),
+        ("ts", [b"2024-03-%02dT12:%02d:%02d.%03dZ" % (1 + i % 28, i % 60, (i * 7) % 60, i % 1000) for i in range(n)]),
+        ("lvl", [[b"info", b"warn", b"error", b"ERROR", b"debug"][i % 5] for i in range(n)]),
+        ("cst", [b"same value"] * n),
+        ("msg", [b"row %d has status %d" % (i, 200 + i % 5) for i in range(n)]),
+    ]
+
+
+def float64_columns(n=300):
+    """a float64 column (f) next to a string column (k)"""
+    fvals = [b"%d.%d" % (i * 7 - 900, i % 97) for i in range(n - 8)] + [b"9007199254740991", b"0.00000015", b"-0.000123", b"123456789.125", b"0.5", b"-12.25", b"12.50", b"125"]
+    return [("f", fvals), ("k", [b"k%d" % i for i in range(n)])]
+
+
 def gpu_rows(ctx, flt, blocks, stage="ondisk"):
     """run the product end to end through vlscan_scan_batch -> list of matching row lists, counts, stats"""
     hb = host_blocks_from_oracle(blocks, stage)

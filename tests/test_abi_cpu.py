@@ -418,38 +418,19 @@ def test_typed_needles_match_oracle(oracle):
 def test_regexp_automaton_matches_oracle(oracle):
     """The compiled form of a regexp leaf - prefix / suffix split plus the rune-class DFA with delayed assertions, in its host mirror
     (what const and dict values are matched with; the kernels step the same tables) - against the oracle's Pike VM on random expressions
-    of the supported syntax and random subjects (UTF-8, newlines, an invalid byte)."""
+    of the supported syntax and random subjects (UTF-8, newlines, an invalid byte).  The leaf's bloom tokens (GetLiterals through
+    skipFirstLastToken) must be the oracle's: one token too many drops blocks that hold matching rows.  The family expressions of
+    tests/regexp_gen.py (the shapes each device strategy is chosen for) go through the same two checks."""
     import random
+    import regexp_gen
     rng = random.Random(7)
-    atoms = ["a", "b", "c", "x", "é", "й", "日", ".", "\\d", "\\w", "\\s", "\\W", "\\D", "[a-c]", "[^a-c]", "[0-9x]", "[[:alpha:]]", "\\.", "\\b", "\\B", "^", "$", "\\A", "\\z",
-             " ", "_", "0", "-", "foo", "bar", "(?i)q", "\\x41", "[é-я]"]
-
-    def gen(depth=0):
-        k = rng.randrange(10)
-        if depth > 3 or k < 4:
-            return rng.choice(atoms)
-        if k == 4:
-            return gen(depth + 1) + gen(depth + 1)
-        if k == 5:
-            return "(" + gen(depth + 1) + "|" + gen(depth + 1) + ")"
-        if k == 6:
-            return "(?:" + gen(depth + 1) + ")" + rng.choice(["*", "+", "?", "{2}", "{1,3}", "{0,2}", "*?", "{2,}"])
-        if k == 7:
-            return "(" + gen(depth + 1) + ")" + rng.choice(["*", "+", "?"])
-        if k == 8:
-            return rng.choice([".*", ".+"]) + gen(depth + 1) + rng.choice(["", ".*", ".+"])
-        return rng.choice(["(?i)", "(?s)", "(?m)", "(?-s)", "(?i:", "("]) + gen(depth + 1)
-
     alphabet = ["a", "b", "c", "x", "A", "Q", "q", "é", "É", "й", "日", " ", "\n", "0", "9", "_", "-", ".", "foo", "bar"]
     compared = 0
     for _ in range(1500):
-        rx = gen()
-        rx += ")" * max(0, rx.count("(") - rx.count(")"))
-        try:
-            oracle.regex_match(rx, b"")
-            valid = True
-        except RuntimeError:
-            valid = False
+        rx = regexp_gen.expr(rng)
+        valid = regexp_gen.is_valid(rx)
+        if valid:
+            assert vs.Program(vs.Filter.regexp("f", rx)).leaf_tokens(0) == oracle.Filter.regexp("f", rx).tokens(), rx
         for _ in range(10):
             s = "".join(rng.choice(alphabet) for _ in range(rng.randrange(0, 9))).encode()
             if rng.random() < 0.1:
@@ -464,7 +445,16 @@ def test_regexp_automaton_matches_oracle(oracle):
             assert got is not None, ("the compiler rejects it", rx)
             assert got == oracle.regex_match(rx, s), (rx, s)
             compared += 1
-    assert compared > 10000
+    assert compared == 15000
+    subjects = [b"", b"\n", b"\xff", b"\xe6\x97", "é".encode()] + [w.encode() for w in regexp_gen.WORDS] + regexp_gen.long_rows(3, 60) + regexp_gen.utf8_edge_rows(4)[:60]
+    families = 0
+    for name, exprs in regexp_gen.family_corpus().items():
+        for rx in exprs:
+            assert vs.Program(vs.Filter.regexp("f", rx)).leaf_tokens(0) == oracle.Filter.regexp("f", rx).tokens(), (name, rx)
+            for s in subjects:
+                assert vs.eval_predicate(5, s, rx.encode()) == oracle.regex_match(rx, s), (name, rx, s)
+            families += 1
+    assert families == 12 * len(regexp_gen.FAMILIES)
 
 
 def test_host_entry_points_are_reentrant(oracle):

@@ -125,20 +125,7 @@ def test_random_differential_strings(env):
 
 def test_numeric_and_special_columns(env):
     oracle, vs, pu, ctx = env
-    n = 300
-    cols = [
-        ("u8", [b"%d" % (i % 200) for i in range(n)]),
-        ("u16", [b"%d" % (i * 37 % 60000) for i in range(n)]),
-        ("u32", [b"%d" % (i * 104729 % 4000000000) for i in range(n)]),
-        ("u64", [b"%d" % (i * 1234567890123 + 5000000000) for i in range(n)]),
-        ("i64", [b"%d" % ((i - 150) * 987654321) for i in range(n)]),
-        ("ip", [b"10.%d.%d.%d" % (i % 3, i % 251, (i * 7) % 256) for i in range(n)]),
-        ("ts", [b"2024-03-%02dT12:%02d:%02d.%03dZ" % (1 + i % 28, i % 60, (i * 7) % 60, i % 1000) for i in range(n)]),
-        ("lvl", [[b"info", b"warn", b"error", b"ERROR", b"debug"][i % 5] for i in range(n)]),
-        ("cst", [b"same value"] * n),
-        ("msg", [b"row %d has status %d" % (i, 200 + i % 5) for i in range(n)]),
-    ]
-    blk = oracle.Block.from_columns(cols)
+    blk = oracle.Block.from_columns(pu.numeric_and_special_columns())
     vts = {c.name: c.value_type for c in blk.columns}
     assert (vts[b"u8"], vts[b"u16"], vts[b"u32"], vts[b"u64"], vts[b"i64"], vts[b"ip"], vts[b"ts"], vts[b"lvl"]) == (3, 4, 5, 6, 10, 8, 9, 2)
     F, G = oracle.Filter, vs.Filter
@@ -163,8 +150,7 @@ def test_numeric_and_special_columns(env):
         check(env, [blk], (F.in_(field, vals), G.in_(field, vals)))
     # combinators across column kinds
     # float64 column: phrase / prefix / regexp go through the per-row float -> shortest text formatting on the device
-    fvals = [b"%d.%d" % (i * 7 - 900, i % 97) for i in range(n - 8)] + [b"9007199254740991", b"0.00000015", b"-0.000123", b"123456789.125", b"0.5", b"-12.25", b"12.50", b"125"]
-    fblk = oracle.Block.from_columns([("f", fvals), ("k", [b"k%d" % i for i in range(n)])])
+    fblk = oracle.Block.from_columns(pu.float64_columns())
     assert {c.name: c.value_type for c in fblk.columns}[b"f"] == 7
     for kind, arg in [("phrase", "123"), ("phrase", "-123"), ("phrase", "123.5"), ("phrase", "125"), ("phrase", "."), ("phrase", "-"), ("phrase", "0"), ("phrase", "56"), ("phrase", "9007199254740991"),
                       ("phrase", "00000015"), ("phrase", "0.00000015"), ("phrase", "12.50"), ("phrase", "12.5"), ("prefix", "12"), ("prefix", "-1"), ("prefix", "0.0"), ("prefix", "."), ("prefix", "-"),
