@@ -329,6 +329,26 @@ int vlscan_gather_values(vlscan_ctx* ctx, const char* field, size_t field_len, u
  *   group key: the bucket, then the text of every by-field as vlscan_gather_values yields it (typed values formatted, "" for a field a block does
  *     not have): `200` stored as uint16 in one block and as a string in another is one group.  Keys are compared byte for byte, never by hash.
  *   by_names: canonical field names ("" = _msg), at most VLSCAN_HITS_MAX_BY; "_time" is rejected.  by_names and by_name_lens may be NULL only when nby == 0.
+ *   by_buckets (vlscan_hits_stats_bucketed / vlscan_hits_sums_bucketed; NULL: no by-field has a bucket, the call is vlscan_hits_stats /
+ *     vlscan_hits_sums): `stats by (f:size offset off)`, one entry per by-field, filled from byStatsField: size =
+ *     bucketSize, offset = bucketOffset, calendar = VLSCAN_BUCKET_* of bucketSizeStr (week / month / year; month and year leave size 0),
+ *     enabled = hasBucketConfig().  An enabled by-field keys on its bucketed text (newValuesBucketedForColumn, lib/logstorage/block_result.go:703-1764):
+ *       const value, string row, dict entry   getBucketedValue(text): "" and a text that does not start with 0-9 or '-' stay as they are; else
+ *                                             the first of tryParseInt64 (truncateInt64, int64 text), tryParseFloat64 (truncateFloat64,
+ *                                             marshalFloat64String), TryParseTimestampRFC3339Nano (truncateTimestamp, RFC3339Nano),
+ *                                             tryParseIPv4 (truncateUint32, IPv4 text), tryParseDuration (truncateInt64, marshalDurationString)
+ *                                             that accepts it; a text none accepts stays as it is
+ *       uint8 .. uint64                       truncateUint64(n, uint64(size), uint64(int64(offset))) -> decimal
+ *       int64                                 truncateInt64(n, int64(size), int64(offset)), a size of 0 counting as 1 -> decimal
+ *       float64                               truncateFloat64(f, p10, int64(size * p10), offset), p10 = math.Pow10(-e), e the exponent of
+ *                                             decimal.FromFloat(size) -> marshalFloat64String
+ *       ipv4                                  truncateUint32(n, uint32(size), uint32(int32(offset))) -> IPv4 text
+ *       iso8601                               truncateTimestamp(ts, int64(size), int64(offset), calendar) -> ISO 8601 text
+ *     Unsigned sizes of 0 and signed sizes <= 0 count as 1 except where noted; float -> integer conversions are Go's on amd64.  A typed column
+ *     whose header minimum and maximum fall into one bucket gives every row of its block that bucket (for float64 also when rows are NaN).  A
+ *     bucketed by-field a block lacks is "".  Keys compare bucketed texts byte for byte: `200` stored as uint16 and `250` as a string are one
+ *     group under size 100.  A NaN or infinite size or offset, an unknown calendar and a size whose int64(size * p10) is 0 (the reference
+ *     would divide by zero) fail the call.
  * Output: the groups sorted by bucket, then by the key texts bytewise: out_buckets[g], out_counts[g] (rows), and the texts of group g's by-field
  * f at out_key_bytes[out_key_offsets[g * nby + f], out_key_offsets[g * nby + f + 1]) (out_key_offsets has cap_groups * nby + 1 entries).
  * out_info (may be NULL) = {groups, key bytes, selected rows, blocks whose timestamps were decoded}; it is filled also when the call fails because
@@ -336,6 +356,11 @@ int vlscan_gather_values(vlscan_ctx* ctx, const char* field, size_t field_len, u
  * are counted without decoding their timestamps. */
 enum { VLSCAN_BUCKET_PLAIN = 0, VLSCAN_BUCKET_WEEK = 1, VLSCAN_BUCKET_MONTH = 2, VLSCAN_BUCKET_YEAR = 3 };
 #define VLSCAN_HITS_MAX_BY 4
+typedef struct vlscan_by_bucket {
+    double size, offset;           /* byStatsField.bucketSize, bucketOffset                                                       */
+    uint32_t calendar;             /* VLSCAN_BUCKET_*                                                                             */
+    uint32_t enabled;              /* byStatsField.hasBucketConfig()                                                              */
+} vlscan_by_bucket;
 typedef struct vlscan_hits_query {
     int64_t step, offset;          /* nanoseconds */
     uint32_t calendar;             /* VLSCAN_BUCKET_*                                                                             */
@@ -345,6 +370,9 @@ typedef struct vlscan_hits_query {
 } vlscan_hits_query;
 int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_buckets, uint64_t* out_counts, uint64_t cap_groups, uint8_t* out_key_bytes,
                       uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t out_info[4]);
+/* vlscan_hits_stats with by_buckets: q->nby entries, or NULL */
+int vlscan_hits_stats_bucketed(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan_by_bucket* by_buckets, int64_t* out_buckets, uint64_t* out_counts,
+                               uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t out_info[4]);
 /* ---- `stats by (_time:step offset off, f1, ...) count(), sum(v1), avg(v1), ...` over the selected rows of the last scan --------------------------
  * The grouping of vlscan_hits_stats (same query, same preconditions, same groups in the same order with the same keys and row counts) plus, per
  * group g and value field f, the partial state a stats shard exports for sum(f) and avg(f) (lib/logstorage/stats_sum.go, stats_avg.go):
@@ -365,8 +393,17 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
 int vlscan_hits_sums(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* const* value_names, const size_t* value_name_lens, uint32_t nvalues, int64_t* out_buckets,
                      uint64_t* out_counts, double* out_sums, uint64_t* out_value_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes,
                      uint64_t* out_key_offsets, uint64_t out_info[4]);
+/* vlscan_hits_sums with by_buckets: q->nby entries, or NULL.  The sums follow the bucketed keys: a block whose raw values differ but fall into
+ * one bucket is one group, added through sumValues. */
+int vlscan_hits_sums_bucketed(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan_by_bucket* by_buckets, const char* const* value_names,
+                              const size_t* value_name_lens, uint32_t nvalues, int64_t* out_buckets, uint64_t* out_counts, double* out_sums,
+                              uint64_t* out_value_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes, uint64_t* out_key_offsets,
+                              uint64_t out_info[4]);
 /* The bucket of one timestamp: host build of the routine the hits kernels run per row (truncateTimestamp above).  For tests. */
 int64_t vlscan_truncate_timestamp(int64_t ts, int64_t step, int64_t offset, uint32_t calendar);
+/* The bucketed text of one const, string or dict text s under bucket b (getBucketedValue above): host build of the routine the hits kernels run.
+ * Returns its length (<= 352; no NUL written), -1 when cap is too small, -2 for a bucket vlscan_hits_stats rejects.  b->enabled is ignored.  For tests. */
+int vlscan_bucket_text(const vlscan_by_bucket* b, const void* s, size_t len, char* out, size_t cap);
 /* ---- the N newest selected rows: `/select/logsql/query?limit=N` (app/vlselect/logsql/logsql.go:932-948, 1005-1080 getLastNQueryResults) ---------
  * Same preconditions as the gather calls: the result of the last vlscan_scan_resident of the ctx, whose batch must still be alive.  Every block
  * with selected rows must have been staged with its timestamps.  The call leaves that result as it was: vlscan_fetch_results, the gather calls

@@ -1,10 +1,10 @@
 #!/usr/bin/env python3
-"""Times `stats by (_time:step, fields) count(), sum(status), avg(status)` (vlscan_hits_sums) on one GPU.
+"""Times `stats by (_time:step, fields) count(), sum(status), avg(status)` (vlscan_hits_sums) on one GPU, with plain and bucketed by-fields.
 
     python tools/stats_bench.py [--steps 20] [--warmup 3]
 
 100 M generated rows (2000 per block, `_msg`, `level` (dict), `path`, `status` (uint16) and a timestamps column: row i at VLSCAN_GEN_T0 + i ms)
-stay resident.  For each of two queries it reports the median wall-clock time of the scan alone, of scan + vlscan_hits_sums, and of scan +
+stay resident.  For each of three queries it reports the median wall-clock time of the scan alone, of scan + vlscan_hits_sums, and of scan +
 vlscan_gather_timestamps / vlscan_gather_values + bucketing, parsing and summing in numpy (what a caller does without the aggregation), the
 bytes each path copies back, and whether both paths gave the same groups, rows and counts (and sums within 2^-40 of the host's) on every call.
 Prints one JSON line with the card's name, power limit and SM clock.  Nothing is written to the repository."""
@@ -22,9 +22,11 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 from hits_bench import SEED, smi  # noqa: E402
 
 ROWS = 100_000_000
-QUERIES = (   # (LogsQL, filter, step ns, by-fields, value fields)
-    ('_msg:"error" | stats by (_time:1s) sum(status), avg(status)', lambda F: F.phrase("_msg", "error"), 10 ** 9, (), ("status",)),
-    ("* | stats by (_time:1h, level) count(), avg(status)", lambda F: F.noop(), 3600 * 10 ** 9, ("level",), ("status",)),
+QUERIES = (   # (LogsQL, filter, step ns, by-fields, value fields, by-field buckets)
+    ('_msg:"error" | stats by (_time:1s) sum(status), avg(status)', lambda F: F.phrase("_msg", "error"), 10 ** 9, (), ("status",), None),
+    ("* | stats by (_time:1h, level) count(), avg(status)", lambda F: F.noop(), 3600 * 10 ** 9, ("level",), ("status",), None),
+    # a dashboard panel `| stats by (status:100) count(), avg(status)` as /select/logsql/stats_query_range sends it
+    ("* | stats by (_time:1h, status:100) count(), avg(status)", lambda F: F.noop(), 3600 * 10 ** 9, ("status",), ("status",), [(100.0, 0.0, 0)]),
 )
 
 
@@ -66,11 +68,19 @@ def workload(ctx, vs, np, steps, warmup, rows=ROWS):
     d_sums, d_vcounts = np.zeros(cap_groups * 4, dtype=np.float64), np.zeros(cap_groups * 4, dtype=np.uint64)
     d_keys, d_offs, d_info = np.zeros(cap_bytes, dtype=np.uint8), np.zeros(cap_groups * 4 + 1, dtype=np.uint64), (C.c_uint64 * 4)()
 
-    def device_path(step, by, values):
+    def decimal(p, lens):   # the packed decimal integer texts -> their values
+        num = np.zeros(lens.size, dtype=np.float64)
+        for k in range(8):   # most significant byte first
+            m = lens > k
+            num[m] = num[m] * 10 + ((p[m] >> np.uint64(8 * (7 - k))) & np.uint64(0xFF)).astype(np.float64) - 48
+        return num
+
+    def device_path(step, by, values, buckets):
         q, keep = vs.hits_query(step, 0, 0, by)
+        bks = vs.by_buckets(buckets, len(by))
         vn = [v.encode() for v in values]
         varr, vlens = (C.c_char_p * len(vn))(*vn), (C.c_size_t * len(vn))(*[len(v) for v in vn])
-        ctx._check(L.vlscan_hits_sums(ctx.h, C.byref(q), varr, vlens, C.c_uint32(len(vn)), d_buckets.ctypes.data_as(C.c_void_p), d_counts.ctypes.data_as(C.c_void_p),
+        ctx._check(L.vlscan_hits_sums_bucketed(ctx.h, C.byref(q), bks, varr, vlens, C.c_uint32(len(vn)), d_buckets.ctypes.data_as(C.c_void_p), d_counts.ctypes.data_as(C.c_void_p),
                                       d_sums.ctypes.data_as(C.c_void_p), d_vcounts.ctypes.data_as(C.c_void_p), C.c_uint64(cap_groups),
                                       d_keys.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes), d_offs.ctypes.data_as(C.c_void_p), d_info))
         g, nby, nv = int(d_info[0]), len(by), len(vn)
@@ -81,32 +91,33 @@ def workload(ctx, vs, np, steps, warmup, rows=ROWS):
         return [(int(buckets[i]), tuple(raw[int(offs[i * nby + f]):int(offs[i * nby + f + 1])] for f in range(nby)), int(counts[i]), float(sums[i]), int(vcounts[i]))
                 for i in range(g)]
 
-    def host_path(step, by, values):
+    def host_path(step, by, values, buckets):
         """gather `_time`, the by-field and the value field; `status` texts are decimal integers here (a uint16 column), so int parsing
-        stands for tryParseFloat64"""
+        stands for tryParseFloat64, and a bucketed `status` is truncateUint64 of that integer"""
         ts, _ = ctx.gather_timestamps(batch)
         d2h = 8 * ts.size + 8 * (nb + 1)
         bucket = ts - np.mod(ts, step)
         b0 = int(bucket.min()) if ts.size else 0
         bidx = (bucket - b0) // step
         code, texts = np.zeros(ts.size, dtype=np.int64), [()]
-        for f in by:
+        for f, bk in zip(by, buckets or [None] * len(by)):
             buf, offs, nbytes = gather_texts(f)
             d2h += nbytes
-            p, _ = packed(buf, offs)
-            uniq, inv = np.unique(p, return_inverse=True)
-            first = np.zeros(uniq.size, dtype=np.int64)
-            first[inv[::-1]] = np.arange(ts.size)[::-1]
-            names = [bytes(buf[int(offs[j]):int(offs[j + 1])]) for j in first]
+            p, lens = packed(buf, offs)
+            if bk:
+                v = decimal(p, lens).astype(np.int64)
+                uniq, inv = np.unique(v - v % int(bk[0]), return_inverse=True)
+                names = [b"%d" % u for u in uniq]
+            else:
+                uniq, inv = np.unique(p, return_inverse=True)
+                first = np.zeros(uniq.size, dtype=np.int64)
+                first[inv[::-1]] = np.arange(ts.size)[::-1]
+                names = [bytes(buf[int(offs[j]):int(offs[j + 1])]) for j in first]
             code = code * uniq.size + inv
             texts = [t + (nm,) for t in texts for nm in names]
         buf, offs, nbytes = gather_texts(values[0])
         d2h += nbytes
-        p, lens = packed(buf, offs)
-        num = np.zeros(ts.size, dtype=np.float64)
-        for k in range(8):   # decimal digits of the packed text, most significant byte first
-            m = lens > k
-            num[m] = num[m] * 10 + ((p[m] >> np.uint64(8 * (7 - k))) & np.uint64(0xFF)).astype(np.float64) - 48
+        num = decimal(*packed(buf, offs))
         ncodes = len(texts)
         key = bidx * ncodes + code
         cnt = np.bincount(key)
@@ -123,7 +134,7 @@ def workload(ctx, vs, np, steps, warmup, rows=ROWS):
 
     out = {"rows": int(batch.rows), "blocks": nb, "note": "times are the median wall-clock time per call including the scan, its synchronisation and the copies "
            "back into preallocated arrays (turning the groups into Python objects is not timed)"}
-    for logsql, tree, step, by, values in QUERIES:
+    for logsql, tree, step, by, values, buckets in QUERIES:
         prog = vs.Program(tree(vs.Filter))
         res = {}
 
@@ -144,10 +155,10 @@ def workload(ctx, vs, np, steps, warmup, rows=ROWS):
             return statistics.median(ms), outs
 
         res["scan_ms"], _ = timed(scan, steps, warmup)
-        res["scan_hits_sums_ms"], dev = timed(lambda: (scan(), device_path(step, by, values))[1], steps, warmup)
+        res["scan_hits_sums_ms"], dev = timed(lambda: (scan(), device_path(step, by, values, buckets))[1], steps, warmup)
         groups, key_bytes, selected = int(d_info[0]), int(d_info[1]), int(d_info[2])
         host_steps = max(1, min(steps, 3))
-        res["scan_gather_numpy_ms"], host = timed(lambda: (scan(), host_path(step, by, values))[1], host_steps, 1)
+        res["scan_gather_numpy_ms"], host = timed(lambda: (scan(), host_path(step, by, values, buckets))[1], host_steps, 1)
         want = device_list(dev[0])
         res["equal"] = all(device_list(d) == want for d in dev) and all(same(want, host_list(h)) for h in host)
         res["groups"] = groups

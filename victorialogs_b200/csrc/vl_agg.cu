@@ -26,6 +26,76 @@ struct Carve {
     size_t place(DevBuf& buf) { buf.ensure(std::max<size_t>(off, 16)); for (auto& f : set) f(buf.as<uint8_t>()); return off; }
 };
 
+// ---- the by-field buckets: the query's size and offset converted as the reference converts them (include/vlscan.h, vlscan_hits_stats) --------
+// Go's float -> integer conversions on amd64: int64 and int32 by CVTTSD2SQ / CVTTSD2SL (NaN and out of range -> the minimum), uint32 through
+// int64, uint64 by the compiler's split at 2^63.
+int32_t go_int32_of_float(double f) { return f > -2147483649.0 && f < 2147483648.0 ? (int32_t)f : INT32_MIN; }
+uint64_t go_uint64_of_float(double f) {
+    const double c = 9223372036854775808.0;
+    return f < c ? (uint64_t)mn::int64_of_float(f) : (uint64_t)mn::int64_of_float(f - c) | (1ull << 63);
+}
+// math.Pow10
+double go_pow10(int n) {
+    static const double tab[32] = {1e0, 1e1, 1e2, 1e3, 1e4, 1e5, 1e6, 1e7, 1e8, 1e9, 1e10, 1e11, 1e12, 1e13, 1e14, 1e15, 1e16, 1e17, 1e18, 1e19, 1e20,
+                                   1e21, 1e22, 1e23, 1e24, 1e25, 1e26, 1e27, 1e28, 1e29, 1e30, 1e31};
+    static const double pos32[10] = {1e0, 1e32, 1e64, 1e96, 1e128, 1e160, 1e192, 1e224, 1e256, 1e288};
+    static const double neg32[11] = {1e-0, 1e-32, 1e-64, 1e-96, 1e-128, 1e-160, 1e-192, 1e-224, 1e-256, 1e-288, 1e-320};
+    if (n >= 0 && n <= 308) return pos32[n / 32] * tab[n % 32];
+    if (n < 0 && n >= -323) return neg32[-n / 32] / tab[-n % 32];
+    return n > 0 ? std::numeric_limits<double>::infinity() : 0.0;
+}
+// the exponent e of decimal.FromFloat(f) = (v, e) for a finite f > 0 (VictoriaMetrics lib/decimal positiveFloatToDecimal, getDecimalAndScale,
+// positiveFloatToDecimalSlow)
+int decimal_exponent(double f) {
+    uint64_t u = go_uint64_of_float(f);
+    int scale = 0;
+    if ((double)u == f) {
+        if (u < (1ull << 55) && u % 10 != 0) return 0;
+        for (; u >= (1ull << 55); u /= 10) scale++;
+        if (u % 10 != 0) return scale;
+        for (u /= 10, scale++; u != 0 && u % 10 == 0; u /= 10) scale++;
+        return scale;
+    }
+    double prec = 1e12;
+    if (f > 1e6 || f < 1e-6) {
+        if (f > 1e6) prec = 1e15;
+        int e2;
+        std::frexp(f, &e2);
+        e2 = std::min(std::max(e2, -1022), 1023);
+        scale = (int16_t)((double)e2 * 0.30102999566398119521);   // math.Ln2 / math.Ln10
+        f *= go_pow10(-scale);
+    }
+    while (f < prec) {
+        double x;
+        const double frac = std::modf(f, &x);
+        if (frac * prec < x) { f = x; break; }
+        if ((1 - frac) * prec < x) { f = x + 1; break; }
+        f *= 100;
+        scale -= 2;
+    }
+    return go_uint64_of_float(f) % 10 != 0 ? scale : scale + 1;
+}
+// BucketSpec of one by-field bucket; an empty string, or why the bucket is rejected
+std::string bucket_spec(const vlscan_by_bucket& b, BucketSpec* o) {
+    if (!std::isfinite(b.size) || !std::isfinite(b.offset)) return "its size and offset must be finite numbers";
+    if (b.calendar > VLSCAN_BUCKET_YEAR) return "unknown calendar bucket kind";
+    memset(o, 0, sizeof *o);
+    o->enabled = 1; o->calendar = b.calendar; o->offset = b.offset;
+    o->u64_size = go_uint64_of_float(b.size); if (o->u64_size == 0) o->u64_size = 1;
+    o->u64_off = (uint64_t)mn::int64_of_float(b.offset);
+    const int64_t i = mn::int64_of_float(b.size);
+    o->i64_size = i <= 0 ? 1 : i;
+    o->i64_col_size = i == 0 ? 1 : i;
+    o->i64_off = mn::int64_of_float(b.offset);
+    o->u32_size = (uint32_t)i; if (o->u32_size == 0) o->u32_size = 1;
+    o->u32_off = (uint32_t)go_int32_of_float(b.offset);
+    const double size = b.size <= 0 ? 1 : b.size;
+    o->p10 = go_pow10(-decimal_exponent(size));
+    o->size_p10 = mn::int64_of_float(size * o->p10);
+    if (o->size_p10 == 0) return "int64(size * 10^-e) is 0 for its float buckets";
+    return "";
+}
+
 }  // namespace
 
 extern "C" {
@@ -131,27 +201,34 @@ static void exclusive_scan(vlscan_ctx* ctx, const uint32_t* lens, uint64_t n, ui
 }
 // texts of column `slot` in the n rows (rows[i], blocks[i]): their lengths and exclusive offsets go to ctx->glens / ctx->goffs (goffs[n] = the
 // total, also returned; synchronises), then text_bytes writes the bytes to ctx->gout
-static uint64_t text_offsets(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint32_t* rows, const uint32_t* blocks, uint64_t n) {
+// `key` (vlscan_hits_stats, a bucketed by-field): the texts come from k_hits_key_texts instead of k_gather_values
+struct HitsKey { HitsQuery q; HitsView V; uint32_t f; };
+static uint64_t text_offsets(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint32_t* rows, const uint32_t* blocks, uint64_t n, const HitsKey* key = nullptr) {
     BatchView B = ctx->last_batch->view();
     ctx->glens.ensure(n * 4); ctx->goffs.ensure((n + 1) * 8);
-    k_gather_values<<<cdiv(n, 128), 128, 0, ctx->stream>>>(B, slot, rows, blocks, n, ro, 0, ctx->glens.as<uint32_t>(), nullptr, nullptr, ctx->gstat.as<unsigned long long>()); launch_check(ctx);
+    if (key) k_hits_key_texts<<<cdiv(n, 128), 128, 0, ctx->stream>>>(B, key->q, key->V, key->f, rows, blocks, n, 0, ctx->glens.as<uint32_t>(), nullptr, nullptr, ctx->gstat.as<unsigned long long>());
+    else k_gather_values<<<cdiv(n, 128), 128, 0, ctx->stream>>>(B, slot, rows, blocks, n, ro, 0, ctx->glens.as<uint32_t>(), nullptr, nullptr, ctx->gstat.as<unsigned long long>());
+    launch_check(ctx);
     exclusive_scan(ctx, ctx->glens.as<uint32_t>(), n, ctx->goffs.as<uint64_t>());
     uint64_t total = 0;
     VL_CUDA(cudaMemcpyAsync(&total, ctx->goffs.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
     check_gather_errors(ctx);
     return total;
 }
-static void text_bytes(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint32_t* rows, const uint32_t* blocks, uint64_t n, uint64_t total) {
+static void text_bytes(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint32_t* rows, const uint32_t* blocks, uint64_t n, uint64_t total, const HitsKey* key = nullptr) {
     ctx->gout.ensure(std::max<uint64_t>(total, 16));
-    k_gather_values<<<cdiv(n, 128), 128, 0, ctx->stream>>>(ctx->last_batch->view(), slot, rows, blocks, n, ro, 1, nullptr, ctx->goffs.as<uint64_t>(), ctx->gout.as<uint8_t>(), ctx->gstat.as<unsigned long long>());
+    if (key) k_hits_key_texts<<<cdiv(n, 128), 128, 0, ctx->stream>>>(ctx->last_batch->view(), key->q, key->V, key->f, rows, blocks, n, 1, nullptr, ctx->goffs.as<uint64_t>(), ctx->gout.as<uint8_t>(),
+                                                                     ctx->gstat.as<unsigned long long>());
+    else k_gather_values<<<cdiv(n, 128), 128, 0, ctx->stream>>>(ctx->last_batch->view(), slot, rows, blocks, n, ro, 1, nullptr, ctx->goffs.as<uint64_t>(), ctx->gout.as<uint8_t>(),
+                                                                ctx->gstat.as<unsigned long long>());
     launch_check(ctx);
 }
 // the texts of column `slot` in the n rows (rows[i], blocks[i]) on the host: text i is bytes[offs[i] .. offs[i + 1])
 static void host_texts(vlscan_ctx* ctx, int slot, const uint32_t* ro, const uint32_t* rows, const uint32_t* blocks, uint64_t n, std::vector<uint64_t>& offs,
-                       std::vector<uint8_t>& bytes) {
-    const uint64_t total = text_offsets(ctx, slot, ro, rows, blocks, n);
+                       std::vector<uint8_t>& bytes, const HitsKey* key = nullptr) {
+    const uint64_t total = text_offsets(ctx, slot, ro, rows, blocks, n, key);
     offs.resize(n + 1); bytes.resize(total);
-    text_bytes(ctx, slot, ro, rows, blocks, n, total);
+    text_bytes(ctx, slot, ro, rows, blocks, n, total, key);
     VL_CUDA(cudaMemcpyAsync(offs.data(), ctx->goffs.p, (n + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
     if (total) VL_CUDA(cudaMemcpyAsync(bytes.data(), ctx->gout.p, total, cudaMemcpyDeviceToHost, ctx->stream));
     check_gather_errors(ctx);   // synchronises
@@ -194,6 +271,16 @@ int vlscan_gather_values(vlscan_ctx* ctx, const char* field, size_t field_len, u
 
 static_assert(VLSCAN_HITS_MAX_BY == VL_HITS_MAX_BY, "the ABI's and the kernels' by-field limits differ");
 int64_t vlscan_truncate_timestamp(int64_t ts, int64_t step, int64_t offset, uint32_t calendar) { return vl::truncate_timestamp(ts, step, offset, calendar); }
+int vlscan_bucket_text(const vlscan_by_bucket* b, const void* s, size_t len, char* out, size_t cap) {
+    BucketSpec bk;
+    if (!b || len > 0xFFFFFFFFu || !bucket_spec(*b, &bk).empty()) return -2;
+    uint8_t buf[VL_FMT_F64_MAX];
+    const uint8_t* p;
+    const uint32_t n = bucket_text(bk, (const uint8_t*)s, (uint32_t)len, buf, &p);
+    if (n > cap) return -1;
+    if (n) memcpy(out, p, n);
+    return (int)n;
+}
 
 static_assert(VLSCAN_STATS_MAX_VALUES == VL_STATS_MAX_VALUES, "the ABI's and the kernels' value-field limits differ");
 // the finished sum of one (group, value field) from its digit sums, frame and flags (k_stats_values): NaN without numbers, as newStatsProcessor
@@ -209,7 +296,7 @@ static double stats_sum(const int64_t d[3], int frame, unsigned flags, uint64_t 
 }
 
 // vlscan_hits_stats (nv == 0) and vlscan_hits_sums: one grouping, then the value sums over the same groups
-static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* const* value_names, const size_t* value_name_lens, uint32_t nv, const char* what,
+static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan_by_bucket* by_buckets, const char* const* value_names, const size_t* value_name_lens, uint32_t nv, const char* what,
                        int64_t* out_buckets, uint64_t* out_counts, double* out_sums, uint64_t* out_value_counts, uint64_t cap_groups, uint8_t* out_key_bytes,
                        uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t out_info[4]) {
     uint64_t info[4] = {0, 0, 0, 0};   // groups, key bytes, selected rows, blocks whose timestamps were decoded
@@ -236,6 +323,13 @@ static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* 
         memset(&hq, 0, sizeof hq);
         hq.step = q->step; hq.offset = q->offset; hq.calendar = q->calendar; hq.nby = q->nby;
         for (uint32_t f = 0; f < q->nby; f++) { hq.slot[f] = b->field_slot(names[f]); hq.row_off8[f] = hit_row_offsets(ctx, hq.slot[f], names[f]); }
+        BucketSpec specs[VL_HITS_MAX_BY];
+        for (uint32_t f = 0; f < q->nby && by_buckets; f++)
+            if (by_buckets[f].enabled) {
+                const std::string why = bucket_spec(by_buckets[f], &specs[f]);
+                if (!why.empty()) throw BadInput("by-field `" + names[f] + "`: bucket rejected: " + why);
+                hq.bucketed |= 1u << f;
+            }
         StatsQuery sq;
         memset(&sq, 0, sizeof sq);
         sq.nv = nv;
@@ -246,14 +340,33 @@ static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* 
         // buckets of the blocks; timestamps decoded only where a block spans several buckets
         unsigned long long* gstat = ctx->gstat.as<unsigned long long>();
         uint32_t* wc = ctx->work_count.as<uint32_t>(); uint32_t* row_blocks = ctx->row_blocks.as<uint32_t>();
-        long long* blk_bucket; uint8_t* blk_multi;
-        Carve().take(blk_bucket, b->nblocks).take(blk_multi, b->nblocks).place(ctx->hblk);
+        long long* blk_bucket; uint8_t* blk_multi; uint8_t* by_fast; unsigned long long* by_lo; BucketSpec* d_specs; KeyTexts* d_keys;
+        Carve().take(blk_bucket, b->nblocks).take(blk_multi, b->nblocks).take(by_fast, b->nblocks * q->nby).take(by_lo, b->nblocks * q->nby).take(d_specs, VL_HITS_MAX_BY)
+            .take(d_keys, VL_HITS_MAX_BY).place(ctx->hblk);
+        if (hq.bucketed) VL_CUDA(cudaMemcpyAsync(d_specs, specs, sizeof specs, cudaMemcpyHostToDevice, ctx->stream));
+        hq.buckets = d_specs;
         VL_CUDA(cudaMemsetAsync(wc, 0, WC_COUNT * 4, ctx->stream));
-        k_hits_classify<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), hq, blk_bucket, blk_multi, row_blocks, wc, gstat); launch_check(ctx);
+        k_hits_classify<<<cdiv(b->nblocks, 256), 256, 0, ctx->stream>>>(B, ctx->counts.as<uint32_t>(), hq, blk_bucket, blk_multi, by_fast, by_lo, row_blocks, wc, gstat);
+        launch_check(ctx);
         const unsigned long long* ts_vals = decode_listed_timestamps(ctx, B, row_blocks, wc);
         uint32_t decoded = 0;
         VL_CUDA(cudaMemcpyAsync(&decoded, wc + WC_ROW, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        HitsView V{ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), blk_bucket, blk_multi, ts_vals};
+        HitsView V{ctx->hits.as<uint32_t>(), ctx->hit_block.as<uint32_t>(), blk_bucket, blk_multi, ts_vals, by_fast, by_lo, d_keys};
+        KeyTexts keys[VL_HITS_MAX_BY] = {};
+        // the bucketed texts of every hit, kept in ctx->ftxt for the grouping pass
+        if (ctx->ftxt.size() < q->nby) ctx->ftxt.resize(q->nby);
+        for (uint32_t f = 0; f < q->nby; f++) {
+            if (!(hq.bucketed >> f & 1)) continue;
+            const HitsKey key{hq, V, f};
+            const uint64_t total = text_offsets(ctx, hq.slot[f], hq.row_off8[f], V.hits, V.hit_block, n, &key);
+            text_bytes(ctx, hq.slot[f], hq.row_off8[f], V.hits, V.hit_block, n, total, &key);
+            DevBuf& T = ctx->ftxt[f];
+            T.ensure((n + 1) * 8 + total + 16);
+            VL_CUDA(cudaMemcpyAsync(T.p, ctx->goffs.p, (n + 1) * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+            if (total) VL_CUDA(cudaMemcpyAsync(T.as<uint8_t>() + (n + 1) * 8, ctx->gout.p, total, cudaMemcpyDeviceToDevice, ctx->stream));
+            keys[f] = KeyTexts{T.as<uint64_t>(), T.as<uint8_t>() + (n + 1) * 8};
+        }
+        if (hq.bucketed) VL_CUDA(cudaMemcpyAsync(d_keys, keys, sizeof keys, cudaMemcpyHostToDevice, ctx->stream));
         // the group table: starts small, grows by 8x while a pass overflows; at 2 x the hit count it cannot overflow
         uint64_t max_cap = 1024; while (max_cap < 2 * n) max_cap <<= 1;
         uint64_t cap = std::min<uint64_t>(max_cap, 1 << 14);
@@ -303,7 +416,8 @@ static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* 
         std::vector<std::vector<uint64_t>> toffs(q->nby); std::vector<std::vector<uint8_t>> tbytes(q->nby);
         uint64_t key_bytes = 0;
         for (uint32_t f = 0; f < q->nby; f++) {
-            host_texts(ctx, hq.slot[f], hq.row_off8[f], rep_rows, rep_blocks, G, toffs[f], tbytes[f]);
+            const HitsKey key{hq, V, f};
+            host_texts(ctx, hq.slot[f], hq.row_off8[f], rep_rows, rep_blocks, G, toffs[f], tbytes[f], (hq.bucketed >> f & 1) ? &key : nullptr);
             key_bytes += tbytes[f].size();
         }
         VL_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -336,18 +450,30 @@ static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* 
 
 int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_buckets, uint64_t* out_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes,
                       uint64_t* out_key_offsets, uint64_t out_info[4]) {
-    return hits_groups(ctx, q, nullptr, nullptr, 0, "vlscan_hits_stats", out_buckets, out_counts, nullptr, nullptr, cap_groups, out_key_bytes, cap_key_bytes, out_key_offsets, out_info);
+    return vlscan_hits_stats_bucketed(ctx, q, nullptr, out_buckets, out_counts, cap_groups, out_key_bytes, cap_key_bytes, out_key_offsets, out_info);
+}
+int vlscan_hits_stats_bucketed(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan_by_bucket* by_buckets, int64_t* out_buckets, uint64_t* out_counts,
+                               uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t out_info[4]) {
+    return hits_groups(ctx, q, by_buckets, nullptr, nullptr, 0, "vlscan_hits_stats", out_buckets, out_counts, nullptr, nullptr, cap_groups, out_key_bytes, cap_key_bytes,
+                       out_key_offsets, out_info);
 }
 
 int vlscan_hits_sums(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* const* value_names, const size_t* value_name_lens, uint32_t nvalues, int64_t* out_buckets,
                      uint64_t* out_counts, double* out_sums, uint64_t* out_value_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes,
                      uint64_t* out_key_offsets, uint64_t out_info[4]) {
+    return vlscan_hits_sums_bucketed(ctx, q, nullptr, value_names, value_name_lens, nvalues, out_buckets, out_counts, out_sums, out_value_counts, cap_groups, out_key_bytes,
+                                     cap_key_bytes, out_key_offsets, out_info);
+}
+int vlscan_hits_sums_bucketed(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan_by_bucket* by_buckets, const char* const* value_names,
+                              const size_t* value_name_lens, uint32_t nvalues, int64_t* out_buckets, uint64_t* out_counts, double* out_sums,
+                              uint64_t* out_value_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes, uint64_t* out_key_offsets,
+                              uint64_t out_info[4]) {
     if (nvalues == 0) {   // a query without value fields is vlscan_hits_stats
         if (out_info) memset(out_info, 0, 4 * sizeof(uint64_t));
         return guarded(ctx, [] { throw BadInput("vlscan_hits_sums: no value fields (vlscan_hits_stats counts without them)"); });
     }
-    return hits_groups(ctx, q, value_names, value_name_lens, nvalues, "vlscan_hits_sums", out_buckets, out_counts, out_sums, out_value_counts, cap_groups, out_key_bytes,
-                       cap_key_bytes, out_key_offsets, out_info);
+    return hits_groups(ctx, q, by_buckets, value_names, value_name_lens, nvalues, "vlscan_hits_sums", out_buckets, out_counts, out_sums, out_value_counts, cap_groups,
+                       out_key_bytes, cap_key_bytes, out_key_offsets, out_info);
 }
 
 // the limit-th largest of the n int64 keys (weights: NULL = 1 each) into the radix state st (RS_COUNT words + VL_RADIX_PASSES histograms), on
@@ -469,21 +595,9 @@ int vlscan_last_rows(vlscan_ctx* ctx, const vlscan_last_query* q, int64_t* out_t
     return rc;
 }
 
-// marshalTimestampRFC3339NanoString in UTC: "2006-01-02T15:04:05" (fmt_iso8601's first 19 bytes), the fraction without its trailing zeros, "Z"
 static std::string rfc3339_nano(int64_t ts) {
     uint8_t buf[32];
-    fmt_iso8601(buf, ts);
-    std::string s((const char*)buf, 19);
-    int64_t frac = ts % 1000000000LL;
-    if (frac < 0) frac += 1000000000LL;
-    if (frac) {
-        char f[16];
-        snprintf(f, sizeof f, ".%09lld", (long long)frac);
-        size_t n = strlen(f);
-        while (f[n - 1] == '0') n--;
-        s.append(f, n);
-    }
-    return s + "Z";
+    return std::string((const char*)buf, fmt_rfc3339nano(buf, ts));
 }
 
 int vlscan_facets(vlscan_ctx* ctx, const vlscan_facets_query* q, uint8_t* out_dropped, uint64_t* out_field_offsets, uint64_t* out_hits, uint8_t* out_classes,

@@ -132,12 +132,17 @@ struct HitsQuery {
     uint32_t calendar, nby;
     int slot[VL_HITS_MAX_BY];                   // batch field slot of every by-field; -1: no block of the batch has it
     const uint32_t* row_off8[VL_HITS_MAX_BY];   // k_lens_offsets of that slot
+    uint32_t bucketed;                          // bit f: by-field f has a bucket, buckets[f] (device memory: a kernel parameter passed on by
+    const BucketSpec* buckets;                  // reference to the noinline reader would be copied to the stack first)
 };
 struct HitsView {
     const uint32_t* hits; const uint32_t* hit_block;                 // build_hit_list
     const long long* blk_bucket; const uint8_t* blk_multi;           // k_hits_classify
     const unsigned long long* ts_vals;                               // k_ts_decode_list of the multi-bucket blocks
+    const uint8_t* by_fast; const unsigned long long* by_lo;         // k_hits_classify, [block * nby + by-field]: typed_header_bucket
+    const struct KeyTexts* keys;                                     // [nby], device memory: the texts of every hit of the bucketed by-fields
 };
+struct KeyTexts { const uint64_t* offs; const uint8_t* bytes; };     // the text of hit h: bytes[offs[h] .. offs[h + 1]) (k_hits_key_texts)
 struct HitsTable {
     unsigned long long* tags;    // [mask + 1]: 0 = empty, else (key hash >> 32) << 32 | (representative hit + 1)
     unsigned long long* cnt;     // [mask + 1]
@@ -148,11 +153,20 @@ struct HitsTable {
 };
 
 // Blocks with hits: the buckets of their minimum and maximum timestamps.  Where they are equal every row of the block is in that bucket (the
-// fast path of getBucketedTimestampValues :769-783) and the timestamps are never decoded; the others go into the decode list.
+// fast path of getBucketedTimestampValues :769-783) and the timestamps are never decoded; the others go into the decode list.  Likewise for every
+// bucketed by-field stored as a typed column: by_fast = the header fast path of its kind holds, by_lo = the block's bucket then.
 static __global__ void k_hits_classify(BatchView B, const uint32_t* __restrict__ counts, HitsQuery q, long long* __restrict__ blk_bucket, uint8_t* __restrict__ blk_multi,
-                                       uint32_t* __restrict__ row_blocks, uint32_t* __restrict__ work_count, unsigned long long* __restrict__ stats) {
+                                       uint8_t* __restrict__ by_fast, unsigned long long* __restrict__ by_lo, uint32_t* __restrict__ row_blocks,
+                                       uint32_t* __restrict__ work_count, unsigned long long* __restrict__ stats) {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B.nblocks || counts[b] == 0) return;
+    for (uint32_t f = 0; f < q.nby; f++) {
+        if (!(q.bucketed >> f & 1)) continue;
+        const DevColumn* c = cell_at(B, q.slot[f], b);
+        uint64_t lo = 0;
+        by_fast[(uint64_t)b * q.nby + f] = cell_typed(c) && typed_header_bucket(*c, q.buckets[f], &lo);
+        by_lo[(uint64_t)b * q.nby + f] = lo;
+    }
     if (!B.ts || B.ts[b].mt == 0) { blk_bucket[b] = 0; blk_multi[b] = 0; atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_NO_TIMESTAMPS); return; }
     const int64_t lo = truncate_timestamp(B.ts[b].first, q.step, q.offset, q.calendar), hi = truncate_timestamp(B.ts[b].max, q.step, q.offset, q.calendar);
     blk_bucket[b] = lo; blk_multi[b] = lo != hi;
@@ -198,23 +212,35 @@ static __device__ __forceinline__ uint32_t warp_run_end(bool valid, bool merge, 
     const uint32_t head = 31 - __clz(heads & (0xffffffffu >> (31 - lane)));
     return lane - head + 1;
 }
-static __device__ uint64_t hits_key_hash(const BatchView& B, const HitsQuery& q, int64_t bucket, uint32_t b, uint32_t r, unsigned long long* stats) {
+// the key text of by-field f in hit h = row r of block b: cell_text, or the bucketed text gathered before the pass (no bucketing code runs in
+// the grouping kernels: called from them, it made them spill four times as much)
+static __device__ __forceinline__ uint32_t by_text(const BatchView& B, const HitsQuery& q, const HitsView& V, uint32_t f, uint64_t h, uint32_t b, uint32_t r, uint8_t* buf,
+                                                   const uint8_t** p, uint32_t* n) {
+    if (q.bucketed >> f & 1) {
+        const KeyTexts& t = V.keys[f];
+        *p = t.bytes + t.offs[h]; *n = (uint32_t)(t.offs[h + 1] - t.offs[h]);
+        return ERR_NONE;
+    }
+    return cell_text(B, cell_at(B, q.slot[f], b), b, r, q.row_off8[f], buf, p, n);
+}
+static __device__ uint64_t hits_key_hash(const BatchView& B, const HitsQuery& q, const HitsView& V, int64_t bucket, uint64_t hit, uint32_t b, uint32_t r, unsigned long long* stats) {
     uint64_t h = mix64((uint64_t)bucket);
     uint8_t buf[VL_FMT_F64_MAX];
     for (uint32_t f = 0; f < q.nby; f++) {
         const uint8_t* src; uint32_t len;
-        report_error(stats, cell_text(B, cell_at(B, q.slot[f], b), b, r, q.row_off8[f], buf, &src, &len));
+        report_error(stats, by_text(B, q, V, f, hit, b, r, buf, &src, &len));
         h = (h ^ len) * 0x100000001B3ull;
         for (uint32_t k = 0; k < len; k++) h = (h ^ src[k]) * 0x100000001B3ull;
         h = mix64(h);
     }
     return h;
 }
-static __device__ bool hits_same_texts(const BatchView& B, const HitsQuery& q, uint32_t b1, uint32_t r1, uint32_t b2, uint32_t r2, unsigned long long* stats) {
+static __device__ bool hits_same_texts(const BatchView& B, const HitsQuery& q, const HitsView& V, uint64_t h1, uint32_t b1, uint32_t r1, uint64_t h2, uint32_t b2, uint32_t r2,
+                                       unsigned long long* stats) {
     uint8_t buf1[VL_FMT_F64_MAX], buf2[VL_FMT_F64_MAX];
     for (uint32_t f = 0; f < q.nby; f++) {
         const uint8_t *s1, *s2; uint32_t l1, l2;
-        report_error(stats, max(cell_text(B, cell_at(B, q.slot[f], b1), b1, r1, q.row_off8[f], buf1, &s1, &l1), cell_text(B, cell_at(B, q.slot[f], b2), b2, r2, q.row_off8[f], buf2, &s2, &l2)));
+        report_error(stats, max(by_text(B, q, V, f, h1, b1, r1, buf1, &s1, &l1), by_text(B, q, V, f, h2, b2, r2, buf2, &s2, &l2)));
         if (l1 != l2) return false;
         for (uint32_t k = 0; k < l1; k++) if (s1[k] != s2[k]) return false;
     }
@@ -225,11 +251,11 @@ static __device__ bool hits_same_texts(const BatchView& B, const HitsQuery& q, u
 static __device__ uint32_t hits_insert(const BatchView& B, const HitsQuery& q, const HitsView& V, const HitsTable& T, int64_t bucket, uint64_t hit, uint32_t b, uint32_t r, uint64_t c,
                                        unsigned long long* stats) {
     if (*(volatile unsigned long long*)&T.state[1]) return 0;
-    const uint64_t hash = hits_key_hash(B, q, bucket, b, r, stats);
+    const uint64_t hash = hits_key_hash(B, q, V, bucket, hit, b, r, stats);
     uint64_t at = 0;
     const int got = key_table_add(T.tags, T.cnt, T.mask, hash, hit, c, [&](uint64_t rep) {
         const uint32_t rb = V.hit_block[rep], rr = V.hits[rep];
-        return hit_bucket(B, q, V, rb, rr) == bucket && hits_same_texts(B, q, b, r, rb, rr, stats);
+        return hit_bucket(B, q, V, rb, rr) == bucket && hits_same_texts(B, q, V, hit, b, r, rep, rb, rr, stats);
     }, [] { return true; }, &at);
     if (got == KEY_NOT_PLACED || (got == KEY_CLAIMED && atomicAdd(&T.state[0], 1ull) >= T.limit)) atomicExch(&T.state[1], 1ull);
     return (uint32_t)at;
@@ -256,7 +282,7 @@ static __global__ void __launch_bounds__(256, SLOTS ? 3 : 4) k_hits_group(BatchV
             stride[f] = codes; ids[f] = nullptr;
             if (q.slot[f] < 0) continue;
             const DevColumn& c = B.cols[(uint64_t)b * B.nfields + q.slot[f]];
-            if (c.kind != COL_VALUES) continue;
+            if (c.kind != COL_VALUES || ((q.bucketed >> f & 1) && V.by_fast[(uint64_t)b * q.nby + f])) continue;   // one text in the whole block
             const uint32_t width = c.dict_len ? c.dict_len : 1;
             ids[f] = plain_dict_ids(B, c, B.blk_rows[b]);   // code_of reads ids only while agg holds
             if (!ids[f] || codes * width > VL_HITS_CODES) { agg = false; continue; }
@@ -320,6 +346,22 @@ static __global__ void k_hits_emit(BatchView B, HitsQuery q, HitsView V, HitsTab
     if (T.slot_group) T.slot_group[s] = (uint32_t)g;
     const uint32_t b = V.hit_block[rep], r = V.hits[rep];
     rep_rows[g] = r; rep_blocks[g] = b; buckets[g] = hit_bucket(B, q, V, b, r); out_counts[g] = T.cnt[s];
+}
+
+// The bucketed text of by-field f in the n rows (rows[i], blocks[i]): k_gather_values with cell_text_bucketed.  Run over every hit before the
+// grouping pass (HitsView.key_offs / key_bytes) and over the groups' representatives after it.
+static __global__ void k_hits_key_texts(BatchView B, HitsQuery q, HitsView V, uint32_t f, const uint32_t* __restrict__ rows, const uint32_t* __restrict__ blocks, uint64_t n, int pass,
+                                        uint32_t* __restrict__ lens_out, const uint64_t* __restrict__ offs, uint8_t* __restrict__ out, unsigned long long* __restrict__ stats) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint8_t buf[VL_FMT_F64_MAX];
+    const uint8_t* src; uint32_t len;
+    const uint32_t b = blocks[i];
+    const uint64_t k = (uint64_t)b * q.nby + f;
+    report_error(stats, cell_text_bucketed(B, cell_at(B, q.slot[f], b), b, rows[i], q.row_off8[f], q.buckets + f, V.by_fast[k], V.by_lo[k], buf, &src, &len));
+    if (pass == 0) { lens_out[i] = len; return; }
+    uint8_t* d = out + offs[i];
+    for (uint32_t k = 0; k < len; k++) d[k] = src[k];
 }
 
 // ---- `stats by (_time:step offset off, f1, ...) sum(v...) avg(v...)`: per group and value field the sum and the count of its numbers -------------

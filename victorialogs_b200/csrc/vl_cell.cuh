@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "vl_hd.cuh"
+#include "vl_mathnum.cuh"
 #include "vl_types.h"
 
 namespace vl {
@@ -195,6 +196,54 @@ static __device__ __noinline__ uint32_t cell_text(const BatchView& B, const DevC
     }
     return err;
 }
+// ---- bucketed texts of a by-field (newValuesBucketedForColumn, lib/logstorage/block_result.go:703-739, 935-1764) -----------------------------
+// A typed value v (uint8..uint64 / ipv4 as stored, int64 and iso8601 as int64 bits, float64 as bits) -> its bucket in the same form
+static __device__ __forceinline__ uint64_t typed_bucket(uint32_t vt, const BucketSpec& bk, uint64_t v) {
+    switch (vt) {
+    case VT_INT64: return (uint64_t)trunc_i64((int64_t)v, bk.i64_col_size, bk.i64_off);
+    case VT_FLOAT64: return f64_bits(trunc_f64(f64_of_bits(v), bk));
+    case VT_IPV4: return trunc_u32((uint32_t)v, bk.u32_size, bk.u32_off);
+    case VT_ISO8601: return (uint64_t)truncate_timestamp((int64_t)v, bk.i64_size, bk.i64_off, bk.calendar);
+    }
+    return trunc_u64(v, bk.u64_size, bk.u64_off);
+}
+// The header fast path of the typed kinds: the buckets of the column's minimum and maximum (the header keeps int64 as plain bits, ipv4 in the
+// low 32 bits); when they are equal every row of the block has that bucket.  float64 buckets compare as numbers: a NaN minimum and maximum
+// fall into one finite bucket.
+static __device__ __forceinline__ bool typed_header_bucket(const DevColumn& c, const BucketSpec& bk, uint64_t* lo) {
+    const uint64_t a = typed_bucket(c.vt, bk, c.min_value), z = typed_bucket(c.vt, bk, c.max_value);
+    *lo = a;
+    return c.vt == VT_FLOAT64 ? f64_of_bits(a) == f64_of_bits(z) : a == z;
+}
+// The bucketed text of row r: a typed value truncated (`fast`: the block's bucket `lo` from typed_header_bucket) and formatted into buf
+// (VL_FMT_F64_MAX bytes); any other text through bucket_text.
+static __device__ __noinline__ uint32_t cell_text_bucketed(const BatchView& B, const DevColumn* c, uint32_t b, uint32_t r, const uint32_t* __restrict__ row_off8, const BucketSpec* bk,
+                                                           bool fast, uint64_t lo, uint8_t* buf, const uint8_t** p, uint32_t* n) {
+    const uint8_t* s; uint32_t len;
+    uint32_t err = ERR_NONE;
+    if (!cell_typed(c)) {
+        err = cell_text_raw(B, c, b, r, row_off8, &s, &len);
+        *n = bucket_text(*bk, s, len, buf, p);
+        return err;
+    }
+    uint64_t v = lo;
+    if (!fast) {
+        err = cell_text_raw(B, c, b, r, row_off8, &s, &len);
+        const uint64_t raw = err ? 0 : load_fixed_be(s, len);
+        v = typed_bucket(c->vt, *bk, c->vt == VT_INT64 ? (uint64_t)unzigzag64(raw) : raw);
+    }
+    int k = 0;
+    switch (c->vt) {
+    case VT_INT64: k = fmt_i64(buf, (int64_t)v); break;
+    case VT_FLOAT64: k = fmt_f64(buf, v); break;
+    case VT_IPV4: k = fmt_ipv4(buf, (uint32_t)v); break;
+    case VT_ISO8601: k = fmt_iso8601(buf, (int64_t)v); break;
+    default: k = fmt_u64(buf, v);
+    }
+    *p = buf; *n = err ? 0 : (uint32_t)k;
+    return err;
+}
+
 // The dict ids of a cell in the plain layout, one byte per row (const lens 1, rows bytes of data), which the dict fast paths read directly;
 // NULL for any other cell, whose rows go through the reader.
 static __device__ __forceinline__ const uint8_t* plain_dict_ids(const BatchView& B, const DevColumn& c, uint32_t rows) {

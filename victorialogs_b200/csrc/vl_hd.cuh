@@ -249,6 +249,19 @@ VL_HDN int fmt_iso8601(uint8_t* buf, int64_t nsecs) {
     fmt_pad(buf + 17, (uint32_t)(sod % 60), 2); buf[19] = '.'; fmt_pad(buf + 20, (uint32_t)(rem / 1000000LL), 3); buf[23] = 'Z';
     return 24;
 }
+// marshalTimestampRFC3339NanoString in UTC: "2006-01-02T15:04:05" (fmt_iso8601's first 19 bytes), the fraction without its trailing zeros, "Z"
+VL_HDN int fmt_rfc3339nano(uint8_t* buf, int64_t nsecs) {
+    fmt_iso8601(buf, nsecs);
+    int n = 19;
+    int64_t frac = nsecs % 1000000000LL;
+    if (frac < 0) frac += 1000000000LL;
+    if (frac) {
+        buf[n++] = '.'; fmt_pad(buf + n, (uint32_t)frac, 9); n += 9;
+        while (buf[n - 1] == '0') n--;
+    }
+    buf[n++] = 'Z';
+    return n;
+}
 
 // ---- predicates of the range / length filters ------------------------------------------------------------------------------------------
 // utf8.RuneCountInString (matchLenRange, filter_len_range.go:333-336): every invalid byte counts as one rune

@@ -509,6 +509,103 @@ VLM_HD double parse_math_number(const uint8_t* p, uint32_t n) {
     memcpy(&f, &bits, 8);
     return f;
 }
+// tryParseInt64 values_encoder.go:622-645 (the facets key a '-' text by the same rule, vl_agg.cuh facet_text_key)
+VLM_HD bool parse_i64(Span s, int64_t* out) {
+    if (s.n == 0) return false;
+    const bool minus = s.p[0] == '-';
+    if (minus) s = sub(s, 1);
+    uint64_t n;
+    if (!parse_u64(s, &n)) return false;
+    if (n >= (1ull << 63) && !(minus && n == (1ull << 63))) return false;
+    *out = (int64_t)(minus ? 0 - n : n);
+    return true;
+}
 
 }  // namespace mn
+
+// ---- bucketed by-fields: `stats by (f:size offset off)` (getBucketedValue and the truncations, lib/logstorage/block_result.go:935-1764) --------
+// The query's bucketSize and bucketOffset as every value kind reads them, converted once on the host (vlscan_hits_stats) by Go's float -> integer
+// rules on amd64.  The float steps of trunc_f64 are separate IEEE operations on the device too: a fused multiply-add would round differently.
+struct BucketSpec {
+    uint32_t enabled, calendar;     // calendar: BUCKET_* (bucketSizeStr "week" / "month" / "year")
+    uint64_t u64_size, u64_off;     // uint64(size) with 0 -> 1, uint64(int64(offset)): uint8..uint64 values
+    int64_t i64_size, i64_off;      // int64(size) with <= 0 -> 1, int64(offset): integer and duration texts, timestamps
+    int64_t i64_col_size;           // int64(size) with only 0 -> 1: int64 values (getBucketedInt64Values)
+    uint32_t u32_size, u32_off;     // uint32(size) with 0 -> 1, uint32(int32(offset)): IPv4 values and texts
+    double offset, p10;             // bucketOffset; math.Pow10(-e), e the exponent of decimal.FromFloat(size) (size <= 0 -> 1)
+    int64_t size_p10;               // int64(size * p10), never 0 (the reference would divide by it)
+};
+#ifdef __CUDA_ARCH__
+#define VLB_MUL(a, b) __dmul_rn(a, b)
+#define VLB_ADD(a, b) __dadd_rn(a, b)
+#define VLB_SUB(a, b) __dsub_rn(a, b)
+#define VLB_DIV(a, b) __ddiv_rn(a, b)
+#else
+#define VLB_MUL(a, b) ((a) * (b))
+#define VLB_ADD(a, b) ((a) + (b))
+#define VLB_SUB(a, b) ((a) - (b))
+#define VLB_DIV(a, b) ((a) / (b))
+#endif
+// truncateUint64 :1237-1249, truncateUint32 :1540-1553
+VLM_HD uint64_t trunc_u64(uint64_t n, uint64_t size, uint64_t off) {
+    if (off == 0) return n - n % size;
+    if (off > n) return 0;
+    n -= off;
+    return n - n % size + off;
+}
+VLM_HD uint32_t trunc_u32(uint32_t n, uint32_t size, uint32_t off) { return (uint32_t)trunc_u64(n, size, off); }
+// truncateInt64 :1333-1351, with Go's wrapping int64 arithmetic (and x % -1 == 0, where C leaves INT64_MIN % -1 undefined)
+VLM_HD int64_t trunc_i64(int64_t n, int64_t size, int64_t off) {
+    const uint64_t t = (uint64_t)n - (uint64_t)off;
+    int64_t r = size == -1 ? 0 : (int64_t)t % size;
+    if (r < 0) r = (int64_t)((uint64_t)r + (uint64_t)size);
+    return (int64_t)(t - (uint64_t)r + (uint64_t)off);
+}
+// truncateFloat64 :1438-1456
+VLM_HD double trunc_f64(double f, const BucketSpec& bk) {
+    if (bk.offset != 0) f = VLB_SUB(f, bk.offset);
+    int64_t fp = mn::int64_of_float(floor(VLB_MUL(f, bk.p10)));
+    fp = (int64_t)((uint64_t)fp - (uint64_t)(fp % bk.size_p10));   // size_p10 is > 0 or INT64_MIN
+    const double g = VLB_DIV((double)fp, bk.p10);
+    return bk.offset != 0 ? VLB_ADD(g, bk.offset) : g;
+}
+VLM_HD uint64_t f64_bits(double f) { uint64_t u; memcpy(&u, &f, 8); return u; }
+VLM_HD double f64_of_bits(uint64_t u) { double f; memcpy(&f, &u, 8); return f; }
+// marshalDurationString values_encoder.go:1063-1126 (-nsecs wraps like Go's: INT64_MIN prints as "-")
+VLM_HD int fmt_duration(uint8_t* buf, int64_t nsecs) {
+    if (nsecs == 0) { buf[0] = '0'; return 1; }
+    int n = 0;
+    if (nsecs < 0) { buf[n++] = '-'; nsecs = (int64_t)(0 - (uint64_t)nsecs); }
+    const int64_t S = 1000000000LL, W = 7 * 86400 * S, D = 86400 * S, H = 3600 * S, M = 60 * S;
+    const bool float_secs = nsecs >= S;
+    const int64_t units[4] = {W, D, H, M};
+    const char names[4] = {'w', 'd', 'h', 'm'};
+    for (int k = 0; k < 4; k++)
+        if (nsecs >= units[k]) { const int64_t q = nsecs / units[k]; nsecs -= q * units[k]; n += fmt_u64(buf + n, (uint64_t)q); buf[n++] = (uint8_t)names[k]; }
+    if (nsecs >= S) {
+        if (float_secs) { n += fmt_f64(buf + n, f64_bits(VLB_DIV((double)nsecs, 1e9))); buf[n++] = 's'; return n; }
+        n += fmt_u64(buf + n, (uint64_t)(nsecs / S)); buf[n++] = 's'; nsecs %= S;
+    }
+    if (nsecs >= 1000000) { n += fmt_u64(buf + n, (uint64_t)(nsecs / 1000000)); buf[n++] = 'm'; buf[n++] = 's'; nsecs %= 1000000; }
+    if (nsecs >= 1000) { n += fmt_u64(buf + n, (uint64_t)(nsecs / 1000)); buf[n++] = 0xC2; buf[n++] = 0xB5; buf[n++] = 's'; nsecs %= 1000; }
+    if (nsecs > 0) { n += fmt_u64(buf + n, (uint64_t)nsecs); buf[n++] = 'n'; buf[n++] = 's'; }
+    return n;
+}
+// getBucketedValue :1666-1764: the bucket of a text, written into buf (VL_FMT_F64_MAX bytes), or the text itself when it has none.  Returns the
+// length; *out = buf or s.
+VLM_HD uint32_t bucket_text(const BucketSpec& bk, const uint8_t* s, uint32_t n, uint8_t* buf, const uint8_t** out) {
+    *out = s;
+    if (n == 0 || ((s[0] < '0' || s[0] > '9') && s[0] != '-')) return n;
+    const mn::Span sp{s, n};
+    int64_t i; double f; uint32_t ip; int k;
+    if (mn::parse_i64(sp, &i)) k = fmt_i64(buf, trunc_i64(i, bk.i64_size, bk.i64_off));
+    else if (mn::parse_f64_internal(sp, false, &f)) k = fmt_f64(buf, f64_bits(trunc_f64(f, bk)));
+    else if (mn::parse_rfc3339nano(sp, &i)) k = fmt_rfc3339nano(buf, truncate_timestamp(i, bk.i64_size, bk.i64_off, bk.calendar));
+    else if (mn::parse_ipv4(sp, &ip)) k = fmt_ipv4(buf, trunc_u32(ip, bk.u32_size, bk.u32_off));
+    else if (mn::parse_duration(sp, &i)) k = fmt_duration(buf, trunc_i64(i, bk.i64_size, bk.i64_off));
+    else return n;
+    *out = buf;
+    return (uint32_t)k;
+}
+
 }  // namespace vl

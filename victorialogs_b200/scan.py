@@ -75,6 +75,10 @@ def gen_streams(k):
     return k << GEN_STREAMS_SHIFT
 
 
+class ByBucket(C.Structure):
+    _fields_ = [("size", C.c_double), ("offset", C.c_double), ("calendar", C.c_uint32), ("enabled", C.c_uint32)]
+
+
 class HitsQuery(C.Structure):
     _fields_ = [("step", C.c_int64), ("offset", C.c_int64), ("calendar", C.c_uint32), ("nby", C.c_uint32),
                 ("by_names", C.POINTER(C.c_char_p)), ("by_name_lens", C.POINTER(C.c_size_t))]
@@ -104,7 +108,7 @@ EXPORTS = ["vlscan_device_count", "vlscan_ctx_create", "vlscan_ctx_free", "vlsca
            "vlscan_batch_upload", "vlscan_batch_free", "vlscan_batch_nblocks", "vlscan_batch_rows", "vlscan_batch_words", "vlscan_batch_device_bytes",
            "vlscan_batch_generate", "vlscan_batch_download", "vlscan_host_blocks_get", "vlscan_host_blocks_field", "vlscan_host_blocks_bytes",
            "vlscan_host_blocks_free", "vlscan_host_blocks_compress", "vlscan_zstd_decompress", "vlscan_zstd_inspect", "vlscan_zstd_walk_digest", "vlscan_part_open", "vlscan_part_free", "vlscan_part_header", "vlscan_part_nblocks", "vlscan_part_block_header", "vlscan_part_timestamps",
-           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_hits_sums", "vlscan_truncate_timestamp", "vlscan_last_rows", "vlscan_facets", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch",
+           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_hits_sums", "vlscan_hits_stats_bucketed", "vlscan_hits_sums_bucketed", "vlscan_truncate_timestamp", "vlscan_bucket_text", "vlscan_last_rows", "vlscan_facets", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch",
            "vlscan_scan_batch_keep", "vlscan_stage_selected"]
 
 
@@ -197,12 +201,43 @@ def truncate_timestamp(ts, step, offset=0, calendar=BUCKET_PLAIN):
     return lib().vlscan_truncate_timestamp(ts, step, offset, calendar)
 
 
+def _by_bucket(spec):
+    """None (the by-field's plain text) or (size, offset, calendar) -> vlscan_by_bucket"""
+    if spec is None:
+        return ByBucket(0.0, 0.0, 0, 0)
+    size, offset, calendar = spec
+    return ByBucket(size, offset, calendar, 1)
+
+
+def bucket_text(text, size, offset=0.0, calendar=BUCKET_PLAIN):
+    """The bucketed text of one const, string or dict text (vlscan_bucket_text: host build of the hits kernels' getBucketedValue); ValueError
+    for a bucket vlscan_hits_stats rejects"""
+    text = _b(text)
+    out = C.create_string_buffer(352)
+    L = lib()
+    L.vlscan_bucket_text.argtypes = [C.POINTER(ByBucket), C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t]
+    n = L.vlscan_bucket_text(C.byref(_by_bucket((size, offset, calendar))), text, len(text), out, 352)
+    if n < 0:
+        raise ValueError((size, offset, calendar))
+    return out.raw[:n]
+
+
 def hits_query(step, offset=0, calendar=BUCKET_PLAIN, by=()):
     """-> (vlscan_hits_query, objects that must stay alive while it is used)"""
     names = [_b(f) for f in by]
     arr = (C.c_char_p * max(len(names), 1))(*names)
     lens = (C.c_size_t * max(len(names), 1))(*[len(x) for x in names])
     return HitsQuery(step, offset, calendar, len(names), arr, lens), (arr, lens)
+
+
+def by_buckets(buckets, nby):
+    """the by_buckets argument of vlscan_hits_stats_bucketed / vlscan_hits_sums_bucketed: None (NULL), or one (size, offset, calendar) or None per
+    by-field (`stats by (f:size offset off)`; calendar = BUCKET_WEEK / _MONTH / _YEAR for `f:week` ..., BUCKET_PLAIN otherwise)"""
+    if buckets is None:
+        return None
+    if len(buckets) != nby:
+        raise ValueError("one bucket (or None) per by-field")
+    return (ByBucket * max(nby, 1))(*[_by_bucket(b) for b in buckets])
 
 
 def last_query(limit, fields=(), min_timestamp=None):
@@ -857,12 +892,14 @@ class Ctx:
         raw = out.tobytes()
         return [raw[int(voffs[i]):int(voffs[i + 1])] for i in range(n)], hoffs
 
-    def hits_stats(self, step, offset=0, calendar=BUCKET_PLAIN, by=(), batch=None, info=None):
+    def hits_stats(self, step, offset=0, calendar=BUCKET_PLAIN, by=(), batch=None, info=None, buckets=None):
         """`stats by (_time:step offset off, by...) count()` over the selected rows of the last scan (vlscan_hits_stats)
         -> [(bucket, (key texts as bytes...), count)] sorted by bucket, then by the texts.  `info` (a dict) receives groups, key_bytes,
-        rows (selected) and blocks_decoded (blocks whose timestamps had to be decoded)."""
+        rows (selected) and blocks_decoded (blocks whose timestamps had to be decoded).  buckets: as for by_buckets (not None: through
+        vlscan_hits_stats_bucketed)."""
         batch = batch or getattr(self, "_last", None)
         q, keep = hits_query(step, offset, calendar, by)
+        bks = by_buckets(buckets, len(by))
         nby = len(by)
         out_info = (C.c_uint64 * 4)()
 
@@ -871,8 +908,12 @@ class Ctx:
             counts = np.zeros(cap_groups, dtype=np.uint64)
             offs = np.zeros(cap_groups * nby + 1, dtype=np.uint64)
             kb = np.zeros(max(cap_bytes, 1), dtype=np.uint8)
-            rc = lib().vlscan_hits_stats(self.h, C.byref(q), buckets.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p), C.c_uint64(cap_groups),
-                                         kb.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes), offs.ctypes.data_as(C.c_void_p), out_info)
+            outs = (buckets.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p), C.c_uint64(cap_groups), kb.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes),
+                    offs.ctypes.data_as(C.c_void_p), out_info)
+            if bks is None:
+                rc = lib().vlscan_hits_stats(self.h, C.byref(q), *outs)
+            else:
+                rc = lib().vlscan_hits_stats_bucketed(self.h, C.byref(q), bks, *outs)
             return rc, (buckets, counts, offs, kb)
         buckets, counts, offs, kb = self._call_grown(call, (max(1, min(int(batch.rows) if batch else 0, 1 << 16)), 1 << 16), lambda: out_info[:2])
         if info is not None:
@@ -880,12 +921,13 @@ class Ctx:
         keys = _row_texts(kb.tobytes(), offs, int(out_info[0]), nby)
         return [(int(buckets[g]), keys[g], int(counts[g])) for g in range(int(out_info[0]))]
 
-    def hits_sums(self, step, offset=0, calendar=BUCKET_PLAIN, by=(), values=(), batch=None, info=None):
+    def hits_sums(self, step, offset=0, calendar=BUCKET_PLAIN, by=(), values=(), batch=None, info=None, buckets=None):
         """`stats by (_time:step offset off, by...) count(), sum(v), avg(v)...` over the selected rows of the last scan (vlscan_hits_sums)
         -> [(bucket, (key texts as bytes...), rows, [(sum, count) per value field])] in the order of hits_stats.  A sum is NaN when its count
-        is 0.  `info` as for hits_stats."""
+        is 0.  `info` and buckets as for hits_stats."""
         batch = batch or getattr(self, "_last", None)
         q, keep = hits_query(step, offset, calendar, by)
+        bks = by_buckets(buckets, len(by))
         vn = [_b(f) for f in values]
         varr = (C.c_char_p * max(len(vn), 1))(*vn)
         vlens = (C.c_size_t * max(len(vn), 1))(*[len(x) for x in vn])
@@ -899,9 +941,12 @@ class Ctx:
             vcounts = np.zeros(max(cap_groups * nv, 1), dtype=np.uint64)
             offs = np.zeros(cap_groups * nby + 1, dtype=np.uint64)
             kb = np.zeros(max(cap_bytes, 1), dtype=np.uint8)
-            rc = lib().vlscan_hits_sums(self.h, C.byref(q), varr, vlens, C.c_uint32(nv), buckets.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p),
-                                        sums.ctypes.data_as(C.c_void_p), vcounts.ctypes.data_as(C.c_void_p), C.c_uint64(cap_groups),
-                                        kb.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes), offs.ctypes.data_as(C.c_void_p), out_info)
+            args = (varr, vlens, C.c_uint32(nv), buckets.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p), sums.ctypes.data_as(C.c_void_p),
+                    vcounts.ctypes.data_as(C.c_void_p), C.c_uint64(cap_groups), kb.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes), offs.ctypes.data_as(C.c_void_p), out_info)
+            if bks is None:
+                rc = lib().vlscan_hits_sums(self.h, C.byref(q), *args)
+            else:
+                rc = lib().vlscan_hits_sums_bucketed(self.h, C.byref(q), bks, *args)
             return rc, (buckets, counts, sums, vcounts, offs, kb)
         buckets, counts, sums, vcounts, offs, kb = self._call_grown(call, (max(1, min(int(batch.rows) if batch else 0, 1 << 16)), 1 << 16), lambda: out_info[:2])
         if info is not None:
