@@ -404,6 +404,28 @@ int64_t vlscan_truncate_timestamp(int64_t ts, int64_t step, int64_t offset, uint
 /* The bucketed text of one const, string or dict text s under bucket b (getBucketedValue above): host build of the routine the hits kernels run.
  * Returns its length (<= 352; no NUL written), -1 when cap is too small, -2 for a bucket vlscan_hits_stats rejects.  b->enabled is ignored.  For tests. */
 int vlscan_bucket_text(const vlscan_by_bucket* b, const void* s, size_t len, char* out, size_t cap);
+/* ---- `stats by (_time:step offset off, f1, ...) histogram(v...)` (lib/logstorage/stats_histogram.go) --------------------------------------------
+ * Per group and value field, the numbers counted per vmrange bucket of metrics.Histogram (VictoriaMetrics/metrics histogram.go).  Groups, keys,
+ * rows, their order, by_buckets, value_names and the preconditions and errors are those of vlscan_hits_sums_bucketed (a trailing `*` is rejected:
+ * `histogram(a*)` does not parse).  A number is what both stats_histogram.go paths read: tryParseNumber of a const, string or dict text
+ * (durations, byte sizes, 0x..., 1_000; "" is none), float64(n) of a uint8..uint64 / int64 row, the double of a float64 row; ipv4 and iso8601
+ * rows, a field the block lacks and `_time` give none.  Histogram.Update then skips NaN and v < 0 (not -0) and indexes the rest:
+ *   index 0 = "0...1.000e-09" (Log10(v) + 9 < 0, -0 and +0 included), 1 .. 486 = metrics bucket index + 1, 487 = "1.000e+18...+Inf" (1e18 and +Inf
+ *   included).  Index order is numeric order; vlscan_vmrange_text gives the vmrange text of an index.
+ * Entries: those of (group g, value field f) are out_entry_ranges / out_entry_hits [out_entry_offsets[g * nvalues + f] .. [+ 1]), non-zero
+ * counts only, by ascending index; out_entry_offsets has cap_groups * nvalues + 1 items.  out_info = {groups, key bytes, selected rows, blocks
+ * whose timestamps were decoded, entries, (block, value field) cells counted from their column header alone}, filled also when a capacity is too
+ * small.  The caller merges batches per (group key, value field, index): hits add (victorialogs_b200.scan.vmranges_merge). */
+#define VLSCAN_VMRANGES 488
+int vlscan_hits_vmranges(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan_by_bucket* by_buckets, const char* const* value_names,
+                         const size_t* value_name_lens, uint32_t nvalues, int64_t* out_buckets, uint64_t* out_counts, uint64_t cap_groups,
+                         uint8_t* out_key_bytes, uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t* out_entry_offsets,
+                         uint16_t* out_entry_ranges, uint64_t* out_entry_hits, uint64_t cap_entries, uint64_t out_info[6]);
+/* The vmrange index of one number (Histogram.Update above), -1 for a number it skips: host build of the mapping the kernel runs.  For tests. */
+int vlscan_vmrange_index(double v);
+/* The vmrange text of index 0 .. VLSCAN_VMRANGES - 1 (%.3e ends, initBucketRanges): its length (no NUL written), -1 when cap is too small, -2 for
+ * an index out of range. */
+int vlscan_vmrange_text(uint32_t index, char* buf, size_t cap);
 /* ---- the N newest selected rows: `/select/logsql/query?limit=N` (app/vlselect/logsql/logsql.go:932-948, 1005-1080 getLastNQueryResults) ---------
  * Same preconditions as the gather calls: the result of the last vlscan_scan_resident of the ctx, whose batch must still be alive.  Every block
  * with selected rows must have been staged with its timestamps.  The call leaves that result as it was: vlscan_fetch_results, the gather calls

@@ -1,5 +1,6 @@
 #!/usr/bin/env python3
-"""Times `stats by (_time:step, fields) count(), sum(status), avg(status)` (vlscan_hits_sums) on one GPU, with plain and bucketed by-fields.
+"""Times `stats by (_time:step, fields) count(), sum(status), avg(status)` (vlscan_hits_sums) on one GPU, with plain and bucketed by-fields, and
+`stats by (_time:step, fields) histogram(status)` (vlscan_hits_vmranges).
 
     python tools/stats_bench.py [--steps 20] [--warmup 3]
 
@@ -7,6 +8,8 @@
 stay resident.  For each of three queries it reports the median wall-clock time of the scan alone, of scan + vlscan_hits_sums, and of scan +
 vlscan_gather_timestamps / vlscan_gather_values + bucketing, parsing and summing in numpy (what a caller does without the aggregation), the
 bytes each path copies back, and whether both paths gave the same groups, rows and counts (and sums within 2^-40 of the host's) on every call.
+The two histogram queries are timed the same way against gather + numpy, where numpy maps each distinct value through vlscan_vmrange_index and
+counts per (group, vmrange); their hits must be equal.
 Prints one JSON line with the card's name, power limit and SM clock.  Nothing is written to the repository."""
 import argparse
 import json
@@ -27,6 +30,10 @@ QUERIES = (   # (LogsQL, filter, step ns, by-fields, value fields, by-field buck
     ("* | stats by (_time:1h, level) count(), avg(status)", lambda F: F.noop(), 3600 * 10 ** 9, ("level",), ("status",), None),
     # a dashboard panel `| stats by (status:100) count(), avg(status)` as /select/logsql/stats_query_range sends it
     ("* | stats by (_time:1h, status:100) count(), avg(status)", lambda F: F.noop(), 3600 * 10 ** 9, ("status",), ("status",), [(100.0, 0.0, 0)]),
+)
+VMR_QUERIES = (   # (LogsQL, filter, step ns, by-fields, value field): the shapes of a Grafana heatmap panel
+    ("* | stats by (_time:1h, level) histogram(status)", lambda F: F.noop(), 3600 * 10 ** 9, ("level",), "status"),
+    ('_msg:"error" | stats by (_time:1s) histogram(status)', lambda F: F.phrase("_msg", "error"), 10 ** 9, (), "status"),
 )
 
 
@@ -91,9 +98,8 @@ def workload(ctx, vs, np, steps, warmup, rows=ROWS):
         return [(int(buckets[i]), tuple(raw[int(offs[i * nby + f]):int(offs[i * nby + f + 1])] for f in range(nby)), int(counts[i]), float(sums[i]), int(vcounts[i]))
                 for i in range(g)]
 
-    def host_path(step, by, values, buckets):
-        """gather `_time`, the by-field and the value field; `status` texts are decimal integers here (a uint16 column), so int parsing
-        stands for tryParseFloat64, and a bucketed `status` is truncateUint64 of that integer"""
+    def host_groups(step, by, buckets):
+        """gather `_time` and the by-fields -> (bucket index, first bucket, key code, key texts by code), D2H bytes"""
         ts, _ = ctx.gather_timestamps(batch)
         d2h = 8 * ts.size + 8 * (nb + 1)
         bucket = ts - np.mod(ts, step)
@@ -115,6 +121,12 @@ def workload(ctx, vs, np, steps, warmup, rows=ROWS):
                 names = [bytes(buf[int(offs[j]):int(offs[j + 1])]) for j in first]
             code = code * uniq.size + inv
             texts = [t + (nm,) for t in texts for nm in names]
+        return (bidx, b0, code, texts), d2h
+
+    def host_path(step, by, values, buckets):
+        """gather `_time`, the by-field and the value field; `status` texts are decimal integers here (a uint16 column), so int parsing
+        stands for tryParseFloat64, and a bucketed `status` is truncateUint64 of that integer"""
+        (bidx, b0, code, texts), d2h = host_groups(step, by, buckets)
         buf, offs, nbytes = gather_texts(values[0])
         d2h += nbytes
         num = decimal(*packed(buf, offs))
@@ -166,6 +178,79 @@ def workload(ctx, vs, np, steps, warmup, rows=ROWS):
         res["d2h_bytes_hits_sums"] = 16 * groups + 16 * groups * len(values) + 8 * (groups * len(by) + 1) + key_bytes
         res["d2h_bytes_gather"] = host[0][1]
         res["timed_runs"] = {"scan": steps, "hits_sums": steps, "gather_numpy": host_steps}
+        out[logsql] = res
+    nvr = vs.VMRANGES
+    d_eoffs, d_ranges, d_hits, v_info = np.zeros(cap_groups + 1, dtype=np.uint64), np.zeros(cap_groups * 8, dtype=np.uint16), np.zeros(cap_groups * 8, dtype=np.uint64), (C.c_uint64 * 6)()
+
+    def device_vmr(step, by, value):
+        q, keep = vs.hits_query(step, 0, 0, by)
+        varr, vlens = (C.c_char_p * 1)(value.encode()), (C.c_size_t * 1)(len(value))
+        ctx._check(L.vlscan_hits_vmranges(ctx.h, C.byref(q), None, varr, vlens, C.c_uint32(1), d_buckets.ctypes.data_as(C.c_void_p), d_counts.ctypes.data_as(C.c_void_p),
+                                          C.c_uint64(cap_groups), d_keys.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes), d_offs.ctypes.data_as(C.c_void_p),
+                                          d_eoffs.ctypes.data_as(C.c_void_p), d_ranges.ctypes.data_as(C.c_void_p), d_hits.ctypes.data_as(C.c_void_p), C.c_uint64(d_ranges.size), v_info))
+        g, e, nby = int(v_info[0]), int(v_info[4]), len(by)
+        return (g, d_buckets[:g].copy(), d_counts[:g].copy(), d_keys[:int(v_info[1])].tobytes(), d_offs[:g * nby + 1].copy(), d_eoffs[:g + 1].copy(), d_ranges[:e].copy(),
+                d_hits[:e].copy(), nby)
+
+    def device_vmr_list(r):
+        g, buckets, counts, raw, offs, eoffs, ranges, hits, nby = r
+        return [(int(buckets[i]), tuple(raw[int(offs[i * nby + f]):int(offs[i * nby + f + 1])] for f in range(nby)), int(counts[i]),
+                 tuple((int(ranges[k]), int(hits[k])) for k in range(int(eoffs[i]), int(eoffs[i + 1])))) for i in range(g)]
+
+    def host_vmr(step, by, value):
+        """gather + numpy: the by-field keys of host_groups, the value field's distinct numbers through vlscan_vmrange_index, one bincount"""
+        (bidx, b0, code, texts), d2h = host_groups(step, by, None)
+        buf, offs, nbytes = gather_texts(value)
+        d2h += nbytes
+        uniq, inv = np.unique(decimal(*packed(buf, offs)), return_inverse=True)
+        idx = np.array([vs.vmrange_index(u) for u in uniq.tolist()], dtype=np.int64)[inv]
+        key = bidx * len(texts) + code
+        rows = np.bincount(key)
+        ok = idx >= 0
+        cnt = np.bincount(key[ok] * nvr + idx[ok])
+        nz = np.nonzero(cnt)[0]
+        return (step, b0, len(texts), texts, rows, nz, cnt[nz]), d2h
+
+    def host_vmr_list(r):
+        step, b0, ncodes, texts, rows, nz, cnt = r[0]
+        ents = {}
+        for k, c in zip(nz.tolist(), cnt.tolist()):
+            ents.setdefault(k // nvr, []).append((k % nvr, c))
+        return sorted((b0 + int(i // ncodes) * step, texts[int(i % ncodes)], int(rows[i]), tuple(ents.get(i, ()))) for i in np.nonzero(rows)[0].tolist())
+
+    for logsql, tree, step, by, value in VMR_QUERIES:
+        prog = vs.Program(tree(vs.Filter))
+        res = {}
+
+        def scan():
+            ctx.scan_resident(prog, batch, want_stats=False)
+
+        def timed(fn, k, warm):
+            for _ in range(warm):
+                fn()
+            ctx.sync()
+            ms, outs = [], []
+            for _ in range(k):
+                t0 = time.perf_counter()
+                r = fn()
+                ctx.sync()
+                ms.append(1000 * (time.perf_counter() - t0))
+                outs.append(r)
+            return statistics.median(ms), outs
+
+        res["scan_ms"], _ = timed(scan, steps, warmup)
+        res["scan_hits_vmranges_ms"], dev = timed(lambda: (scan(), device_vmr(step, by, value))[1], steps, warmup)
+        groups, key_bytes, selected, entries = int(v_info[0]), int(v_info[1]), int(v_info[2]), int(v_info[4])
+        host_steps = max(1, min(steps, 3))
+        res["scan_gather_numpy_ms"], host = timed(lambda: (scan(), host_vmr(step, by, value))[1], host_steps, 1)
+        want = device_vmr_list(dev[0])
+        res["equal"] = all(device_vmr_list(d) == want for d in dev) and all(host_vmr_list(h) == want for h in host)
+        res["groups"] = groups
+        res["entries"] = entries
+        res["selected_rows"] = selected
+        res["d2h_bytes_hits_vmranges"] = 16 * groups + 8 * (groups * len(by) + 1) + key_bytes + 16 * entries   # the compacted (key, count) entries
+        res["d2h_bytes_gather"] = host[0][1]
+        res["timed_runs"] = {"scan": steps, "hits_vmranges": steps, "gather_numpy": host_steps}
         out[logsql] = res
     batch.free()
     return out

@@ -1,5 +1,5 @@
 // libvlscan.so: the aggregations over the last scan's result, driven from the host: the hit list and the gathers of values and timestamps
-// (vlscan_fetch_hits, vlscan_gather_*), the hits histogram and its value sums (vlscan_hits_stats, vlscan_hits_sums), the N newest rows
+// (vlscan_fetch_hits, vlscan_gather_*), the hits histogram, its value sums and vmranges (vlscan_hits_stats, _sums, _vmranges), the N newest rows
 // (vlscan_last_rows) and the facets (vlscan_facets).  Their kernels are in vl_agg.cuh; row offsets come from the scan's row_offsets.
 #include <algorithm>
 #include <cmath>
@@ -7,6 +7,7 @@
 #include <cstring>
 #include <functional>
 #include <limits>
+#include <mutex>
 #include <string>
 #include <string_view>
 #include <vector>
@@ -94,6 +95,88 @@ std::string bucket_spec(const vlscan_by_bucket& b, BucketSpec* o) {
     o->size_p10 = mn::int64_of_float(size * o->p10);
     if (o->size_p10 == 0) return "int64(size * 10^-e) is 0 for its float buckets";
     return "";
+}
+
+// ---- the vmrange index of metrics.Histogram.Update (include/vlscan.h, vlscan_hits_vmranges) -----------------------------------------------------
+// Go's portable math.Log (math/log.go: the fdlibm reduction by Frexp, s = f / (2 + f), L1..L7, Ln2Hi / Ln2Lo), every step one rounded double
+// operation.  The amd64 build of Go runs an assembly archLog that mirrors this algorithm; DESIGN §3.15 states that assumption.
+double go_log(double x) {
+    const double Ln2Hi = 6.93147180369123816490e-01, Ln2Lo = 1.90821492927058770002e-10, L1 = 6.666666666666735130e-01, L2 = 3.999999999940941908e-01,
+                 L3 = 2.857142874366239149e-01, L4 = 2.222219843214978396e-01, L5 = 1.818357216161805012e-01, L6 = 1.531383769920937332e-01,
+                 L7 = 1.479819860511658591e-01;
+    if (std::isnan(x) || x == std::numeric_limits<double>::infinity()) return x;
+    if (x < 0) return std::numeric_limits<double>::quiet_NaN();
+    if (x == 0) return -std::numeric_limits<double>::infinity();
+    int ki;
+    double f1 = std::frexp(x, &ki);
+    if (f1 < 0.70710678118654752440) { f1 *= 2; ki--; }   // Sqrt2 / 2
+    const double f = f1 - 1, k = (double)ki;
+    const double s = f / (2 + f), s2 = s * s, s4 = s2 * s2;
+    const double t1 = s2 * (L1 + s4 * (L3 + s4 * (L5 + s4 * L7)));
+    const double t2 = s4 * (L2 + s4 * (L4 + s4 * L6));
+    const double R = t1 + t2, hfsq = 0.5 * f * f;
+    return k * Ln2Hi - ((hfsq - (s * (hfsq + R) + k * Ln2Lo)) - f);
+}
+// Histogram.Update's index from its formula: b = (Log10(v) - e10Min) * bucketsPerDecimal with Log10(x) = Log(x) * (1 / Ln10), 1 / Ln10 the
+// correctly rounded constant; lower below 0, upper from 486, else uint(b), one less when b is an integer above 0 (10^n goes to the bucket below)
+int vmr_index_formula(double v) {
+    if (std::isnan(v) || v < 0) return -1;
+    const double b = (go_log(v) * 0x1.bcb7b1526e50ep-2 - (-9.0)) * 18.0;
+    if (b < 0) return 0;
+    if (b >= 486) return VL_VMRANGES - 1;
+    uint64_t idx = (uint64_t)b;
+    if (b == (double)idx && idx > 0) idx--;
+    return (int)idx + 1;
+}
+double f64_bits(uint64_t u) { double d; memcpy(&d, &u, 8); return d; }
+// bound k - 1 = the least double whose formula index reaches k, found by bisection on the bit patterns of +0 .. +Inf.  The kernels and
+// vmr_index_host search this table, so the device gives the host's index by construction.  Built once; the build checks that the formula does
+// not decrease for 2000 ulps on either side of every bound, where a search over the bounds would disagree with it.
+const std::vector<double>& vmr_bounds() {
+    static std::vector<double> bounds;
+    static std::string error;
+    static std::once_flag once;
+    std::call_once(once, [] {
+        const uint64_t inf = 0x7FF0000000000000ull;
+        for (int k = 1; k < VL_VMRANGES; k++) {
+            uint64_t lo = 0, hi = inf;   // index(lo) < k <= index(hi)
+            while (hi - lo > 1) { const uint64_t m = lo + (hi - lo) / 2; (vmr_index_formula(f64_bits(m)) >= k ? hi : lo) = m; }
+            bounds.push_back(f64_bits(hi));
+            int prev = -1;
+            for (uint64_t u = hi > 2000 ? hi - 2000 : 0; u <= hi + 2000; u++) {
+                const int x = vmr_index_formula(f64_bits(u));
+                if (x < prev) error = "the vmrange index decreases near bound " + std::to_string(k);
+                prev = x;
+            }
+        }
+    });
+    if (!error.empty()) throw BadInput(error);
+    return bounds;
+}
+int vmr_index_host(double v) {
+    if (std::isnan(v) || v < 0) return -1;
+    const std::vector<double>& b = vmr_bounds();
+    return (int)(std::upper_bound(b.begin(), b.end(), v) - b.begin());
+}
+// the vmrange texts by index: lowerBucketRange, bucketRanges (initBucketRanges: v = Pow10(-9), then v *= Pow(10, 1/18) 486 times, each end
+// printed with %.3e), upperBucketRange.  The texts are the same for every multiplier within 16 ulps of 10^(1/18) (a test pins that), so
+// they do not depend on how Go's Pow rounds.
+const std::vector<std::string>& vmr_texts() {
+    static std::vector<std::string> t;
+    static std::once_flag once;
+    std::call_once(once, [] {
+        auto e3 = [](double v) { char b[32]; snprintf(b, sizeof b, "%.3e", v); return std::string(b); };
+        const double mult = std::pow(10.0, 1.0 / 18);
+        double v = go_pow10(-9);
+        t.push_back("0..." + e3(v));
+        for (int i = 0; i < VL_VMRANGES - 2; i++) {
+            const std::string start = e3(v);
+            v *= mult;
+            t.push_back(start + "..." + e3(v));
+        }
+        t.push_back(e3(go_pow10(18)) + "...+Inf");
+    });
+    return t;
 }
 
 }  // namespace
@@ -295,11 +378,24 @@ static double stats_sum(const int64_t d[3], int frame, unsigned flags, uint64_t 
     return std::ldexp((double)t, frame - VL_STATS_FRAME_BIAS - 92);
 }
 
-// vlscan_hits_stats (nv == 0) and vlscan_hits_sums: one grouping, then the value sums over the same groups
+// The value aggregation over the groups of hits_groups (vlscan_hits_sums, vlscan_hits_vmranges).  run: after the groups are emitted, on the
+// device state they leave (copies its results to the host; may set info[4..]).  write: the results in the caller's buffers in group order,
+// after the groups' capacities passed and before the groups are written (a capacity of its own that is too small fails the call).
+struct GroupPass {
+    vlscan_ctx* ctx; const BatchView& B; const StatsQuery& sq; const HitsView& V; const HitsTable& T; uint64_t n, G; unsigned grid; uint64_t* info;
+};
+struct ValueAgg {
+    const char* prefix_example;   // the pipe a prefix value field would be, for the error
+    std::function<void(Carve&, uint64_t G)> take;   // optional: device arrays laid out after the groups' (ctx->hgrp)
+    std::function<void(const GroupPass&)> run;
+    std::function<void(const std::vector<uint64_t>& order)> write;
+};
+
+// vlscan_hits_stats (agg NULL), vlscan_hits_sums and vlscan_hits_vmranges: one grouping, then the value aggregation over the same groups
 static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan_by_bucket* by_buckets, const char* const* value_names, const size_t* value_name_lens, uint32_t nv, const char* what,
-                       int64_t* out_buckets, uint64_t* out_counts, double* out_sums, uint64_t* out_value_counts, uint64_t cap_groups, uint8_t* out_key_bytes,
-                       uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t out_info[4]) {
-    uint64_t info[4] = {0, 0, 0, 0};   // groups, key bytes, selected rows, blocks whose timestamps were decoded
+                       int64_t* out_buckets, uint64_t* out_counts, uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes, uint64_t* out_key_offsets,
+                       uint64_t* out_info, size_t ninfo, const ValueAgg* agg) {
+    uint64_t info[6] = {0, 0, 0, 0, 0, 0};   // groups, key bytes, selected rows, blocks whose timestamps were decoded, then the aggregation's
     const int rc = guarded(ctx, [&] {
         if (!q) throw BadInput("no hits query");
         if (q->calendar > VLSCAN_BUCKET_YEAR) throw BadInput("unknown calendar bucket kind");
@@ -307,10 +403,10 @@ static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan
         const std::vector<std::string> names = canonical_names(q->by_names, q->by_name_lens, q->nby, what);
         for (const std::string& n : names)
             if (n == "_time") throw BadInput("`_time` cannot be a by-field of the hits aggregation: it is the bucket");
-        if (nv > VLSCAN_STATS_MAX_VALUES) throw BadInput("too many value fields for vlscan_hits_sums (at most VLSCAN_STATS_MAX_VALUES = 4)");
+        if (nv > VLSCAN_STATS_MAX_VALUES) throw BadInput(std::string("too many value fields for ") + what + " (at most VLSCAN_STATS_MAX_VALUES = 4)");
         const std::vector<std::string> vnames = canonical_names(value_names, value_name_lens, nv, what);
         for (const std::string& v : vnames)
-            if (v.back() == '*') throw BadInput("value field `" + v + "`: a prefix filter such as sum(foo*) is not supported by vlscan_hits_sums");
+            if (v.back() == '*') throw BadInput("value field `" + v + "`: a prefix filter such as " + agg->prefix_example + " is not supported by " + what);
         if (!ctx) throw BadInput(std::string(what) + " needs a vlscan_ctx on a CUDA device (there is no CPU fallback)");
         const uint64_t n = build_hit_list(ctx, nullptr);
         if (n >= 0xFFFFFFFFull) throw BadInput("more than 2^32 - 2 selected rows in one batch");
@@ -393,23 +489,13 @@ static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan
         info[0] = G; info[3] = decoded;
         // the groups, then the texts of their representatives only
         long long* buckets; unsigned long long* counts; uint32_t* rep_rows; uint32_t* rep_blocks;
-        StatsAcc A;
         Carve cv;
         cv.take(buckets, G).take(counts, G).take(rep_rows, G).take(rep_blocks, G);
-        if (nv) cv.take(T.slot_group, cap).take(A.digits, 3 * G * nv).take(A.count, G * nv).take(A.frame, G * nv).take(A.flags, G * nv);
+        if (nv) cv.take(T.slot_group, cap);
+        if (agg && agg->take) agg->take(cv, G);
         cv.place(ctx->hgrp);
-        if (nv) VL_CUDA(cudaMemsetAsync(A.digits, 0, (uint8_t*)(A.flags + G * nv) - (uint8_t*)A.digits, ctx->stream));
         k_hits_emit<<<cdiv(cap, 256), 256, 0, ctx->stream>>>(B, hq, V, T, rep_rows, rep_blocks, buckets, counts); launch_check(ctx);
-        std::vector<int64_t> hd(3 * G * nv); std::vector<uint64_t> hn(G * nv); std::vector<int> hf(G * nv); std::vector<unsigned> hfl(G * nv);
-        if (nv) {   // the value sums: pass 0 counts and frames, pass 1 digits (k_stats_values)
-            k_stats_values<0><<<grid, 256, 0, ctx->stream>>>(B, sq, V, T.hit_slot, T.slot_group, A, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat); launch_check(ctx);
-            k_stats_values<1><<<grid, 256, 0, ctx->stream>>>(B, sq, V, T.hit_slot, T.slot_group, A, ctx->counts.as<uint32_t>(), ctx->hit_offs.as<uint64_t>(), gstat); launch_check(ctx);
-            VL_CUDA(cudaMemcpyAsync(hd.data(), A.digits, hd.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
-            VL_CUDA(cudaMemcpyAsync(hn.data(), A.count, hn.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
-            VL_CUDA(cudaMemcpyAsync(hf.data(), A.frame, hf.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
-            VL_CUDA(cudaMemcpyAsync(hfl.data(), A.flags, hfl.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
-            check_gather_errors(ctx);
-        }
+        if (agg) agg->run(GroupPass{ctx, B, sq, V, T, n, G, grid, info});
         std::vector<int64_t> hb(G); std::vector<uint64_t> hc(G);
         VL_CUDA(cudaMemcpyAsync(hb.data(), buckets, G * 8, cudaMemcpyDeviceToHost, ctx->stream));
         VL_CUDA(cudaMemcpyAsync(hc.data(), counts, G * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -424,8 +510,7 @@ static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan
         info[1] = key_bytes;
         if (G > cap_groups) throw BadInput("hits groups buffer too small (the needed size is reported)");
         if (key_bytes > cap_key_bytes) throw BadInput("hits key bytes buffer too small (the needed size is reported)");
-        if (!out_buckets || !out_counts || (q->nby && (!out_key_offsets || (key_bytes && !out_key_bytes))) || (nv && (!out_sums || !out_value_counts)))
-            throw BadInput("hits output buffer missing");
+        if (!out_buckets || !out_counts || (q->nby && (!out_key_offsets || (key_bytes && !out_key_bytes)))) throw BadInput("hits output buffer missing");
         // sorted by bucket, then by the key texts bytewise
         std::vector<uint64_t> order(G);
         for (uint64_t g = 0; g < G; g++) order[g] = g;
@@ -435,16 +520,11 @@ static int hits_groups(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan
             for (uint32_t f = 0; f < q->nby; f++) { const int c = text(f, x).compare(text(f, y)); if (c) return c < 0; }
             return false;
         });
+        if (agg) agg->write(order);
         for (uint64_t i = 0; i < G; i++) { out_buckets[i] = hb[order[i]]; out_counts[i] = hc[order[i]]; }
-        for (uint64_t i = 0; i < G; i++)
-            for (uint32_t f = 0; f < nv; f++) {
-                const uint64_t k = order[i] * nv + f;
-                out_sums[i * nv + f] = stats_sum(&hd[3 * k], hf[k], hfl[k], hn[k]);
-                out_value_counts[i * nv + f] = hn[k];
-            }
         pack_texts(order, toffs, tbytes, out_key_bytes, out_key_offsets);
     });
-    if (out_info) memcpy(out_info, info, sizeof info);
+    if (out_info) memcpy(out_info, info, ninfo * sizeof(uint64_t));
     return rc;
 }
 
@@ -454,8 +534,8 @@ int vlscan_hits_stats(vlscan_ctx* ctx, const vlscan_hits_query* q, int64_t* out_
 }
 int vlscan_hits_stats_bucketed(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan_by_bucket* by_buckets, int64_t* out_buckets, uint64_t* out_counts,
                                uint64_t cap_groups, uint8_t* out_key_bytes, uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t out_info[4]) {
-    return hits_groups(ctx, q, by_buckets, nullptr, nullptr, 0, "vlscan_hits_stats", out_buckets, out_counts, nullptr, nullptr, cap_groups, out_key_bytes, cap_key_bytes,
-                       out_key_offsets, out_info);
+    return hits_groups(ctx, q, by_buckets, nullptr, nullptr, 0, "vlscan_hits_stats", out_buckets, out_counts, cap_groups, out_key_bytes, cap_key_bytes, out_key_offsets,
+                       out_info, 4, nullptr);
 }
 
 int vlscan_hits_sums(vlscan_ctx* ctx, const vlscan_hits_query* q, const char* const* value_names, const size_t* value_name_lens, uint32_t nvalues, int64_t* out_buckets,
@@ -472,8 +552,119 @@ int vlscan_hits_sums_bucketed(vlscan_ctx* ctx, const vlscan_hits_query* q, const
         if (out_info) memset(out_info, 0, 4 * sizeof(uint64_t));
         return guarded(ctx, [] { throw BadInput("vlscan_hits_sums: no value fields (vlscan_hits_stats counts without them)"); });
     }
-    return hits_groups(ctx, q, by_buckets, value_names, value_name_lens, nvalues, "vlscan_hits_sums", out_buckets, out_counts, out_sums, out_value_counts, cap_groups,
-                       out_key_bytes, cap_key_bytes, out_key_offsets, out_info);
+    const uint32_t nv = nvalues;
+    std::vector<int64_t> hd; std::vector<uint64_t> hn; std::vector<int> hf; std::vector<unsigned> hfl;
+    ValueAgg agg;
+    agg.prefix_example = "sum(foo*)";
+    StatsAcc A;
+    agg.take = [&](Carve& cv, uint64_t G) { cv.take(A.digits, 3 * G * nv).take(A.count, G * nv).take(A.frame, G * nv).take(A.flags, G * nv); };
+    agg.run = [&](const GroupPass& P) {   // the value sums: pass 0 counts and frames, pass 1 digits (k_stats_values)
+        vlscan_ctx* c = P.ctx;
+        const uint64_t G = P.G;
+        VL_CUDA(cudaMemsetAsync(A.digits, 0, (uint8_t*)(A.flags + G * nv) - (uint8_t*)A.digits, c->stream));
+        unsigned long long* gstat = c->gstat.as<unsigned long long>();
+        k_stats_values<0><<<P.grid, 256, 0, c->stream>>>(P.B, P.sq, P.V, P.T.hit_slot, P.T.slot_group, A, c->counts.as<uint32_t>(), c->hit_offs.as<uint64_t>(), gstat); launch_check(c);
+        k_stats_values<1><<<P.grid, 256, 0, c->stream>>>(P.B, P.sq, P.V, P.T.hit_slot, P.T.slot_group, A, c->counts.as<uint32_t>(), c->hit_offs.as<uint64_t>(), gstat); launch_check(c);
+        hd.resize(3 * G * nv); hn.resize(G * nv); hf.resize(G * nv); hfl.resize(G * nv);
+        VL_CUDA(cudaMemcpyAsync(hd.data(), A.digits, hd.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+        VL_CUDA(cudaMemcpyAsync(hn.data(), A.count, hn.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+        VL_CUDA(cudaMemcpyAsync(hf.data(), A.frame, hf.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+        VL_CUDA(cudaMemcpyAsync(hfl.data(), A.flags, hfl.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+        check_gather_errors(c);
+    };
+    agg.write = [&](const std::vector<uint64_t>& order) {
+        if (!out_sums || !out_value_counts) throw BadInput("hits output buffer missing");
+        for (uint64_t i = 0; i < order.size(); i++)
+            for (uint32_t f = 0; f < nv; f++) {
+                const uint64_t k = order[i] * nv + f;
+                out_sums[i * nv + f] = stats_sum(&hd[3 * k], hf[k], hfl[k], hn[k]);
+                out_value_counts[i * nv + f] = hn[k];
+            }
+    };
+    return hits_groups(ctx, q, by_buckets, value_names, value_name_lens, nvalues, "vlscan_hits_sums", out_buckets, out_counts, cap_groups, out_key_bytes, cap_key_bytes,
+                       out_key_offsets, out_info, 4, &agg);
+}
+
+int vlscan_hits_vmranges(vlscan_ctx* ctx, const vlscan_hits_query* q, const vlscan_by_bucket* by_buckets, const char* const* value_names,
+                         const size_t* value_name_lens, uint32_t nvalues, int64_t* out_buckets, uint64_t* out_counts, uint64_t cap_groups,
+                         uint8_t* out_key_bytes, uint64_t cap_key_bytes, uint64_t* out_key_offsets, uint64_t* out_entry_offsets,
+                         uint16_t* out_entry_ranges, uint64_t* out_entry_hits, uint64_t cap_entries, uint64_t out_info[6]) {
+    if (nvalues == 0) {
+        if (out_info) memset(out_info, 0, 6 * sizeof(uint64_t));
+        return guarded(ctx, [] { throw BadInput("vlscan_hits_vmranges: no value fields (histogram takes one field)"); });
+    }
+    const uint32_t nv = nvalues;
+    std::vector<unsigned long long> ek, ec;                   // the table's entries: key (g * nv + f) * VL_VMRANGES + index, hits
+    std::vector<std::pair<uint16_t, uint64_t>> entries;       // (index, hits) by (device group, value field), then index
+    std::vector<uint64_t> first;                              // the first entry of every (device group, value field)
+    ValueAgg agg;
+    agg.prefix_example = "histogram(foo*)";
+    agg.run = [&](const GroupPass& P) {
+        vlscan_ctx* c = P.ctx;
+        const std::vector<double>& bounds = vmr_bounds();
+        // the vmrange table: starts small, grows by 8x while a pass overflows; at 2 x (hits x value fields) it cannot overflow
+        uint64_t max_cap = 1024; while (max_cap < 2 * P.n * nv) max_cap <<= 1;
+        uint64_t cap = std::min<uint64_t>(max_cap, 1 << 14);
+        VmrTable M;
+        double* d_bounds; unsigned long long* out_keys; unsigned long long* out_cnt;
+        unsigned long long state[4];
+        for (;;) {
+            Carve cv;
+            cv.take(d_bounds, VL_VMR_BOUNDS).take(M.keys, cap).take(M.cnt, cap).take(M.state, 4).take(out_keys, cap).take(out_cnt, cap).place(c->vagg);
+            M.mask = cap - 1; M.limit = cap == max_cap ? cap : cap / 2;
+            VL_CUDA(cudaMemcpyAsync(d_bounds, bounds.data(), VL_VMR_BOUNDS * 8, cudaMemcpyHostToDevice, c->stream));
+            VL_CUDA(cudaMemsetAsync(M.keys, 0, (uint8_t*)(M.state + 4) - (uint8_t*)M.keys, c->stream));
+            k_stats_vmranges<<<P.grid, 256, 0, c->stream>>>(P.B, P.sq, P.V, P.T.hit_slot, P.T.slot_group, d_bounds, M, c->counts.as<uint32_t>(), c->hit_offs.as<uint64_t>(),
+                                                             c->gstat.as<unsigned long long>());
+            launch_check(c);
+            VL_CUDA(cudaMemcpyAsync(state, M.state, sizeof state, cudaMemcpyDeviceToHost, c->stream));
+            VL_CUDA(cudaStreamSynchronize(c->stream));
+            if (!state[1]) break;
+            if (cap == max_cap) throw BadInput("vlscan_hits_vmranges: vmrange table overflow");
+            cap = std::min(cap * 8, max_cap);
+        }
+        const uint64_t E = state[0];
+        k_vmr_compact<<<cdiv(cap, 256), 256, 0, c->stream>>>(M, out_keys, out_cnt); launch_check(c);
+        ek.resize(E); ec.resize(E);
+        if (E) {
+            VL_CUDA(cudaMemcpyAsync(ek.data(), out_keys, E * 8, cudaMemcpyDeviceToHost, c->stream));
+            VL_CUDA(cudaMemcpyAsync(ec.data(), out_cnt, E * 8, cudaMemcpyDeviceToHost, c->stream));
+        }
+        check_gather_errors(c);   // synchronises
+        P.info[4] = E; P.info[5] = state[3];
+        // by (device group, value field) with a counting pass, then by index inside each of them (at most VL_VMRANGES entries)
+        first.assign(P.G * nv + 1, 0);
+        for (uint64_t e = 0; e < E; e++) first[ek[e] / VL_VMRANGES + 1]++;
+        for (size_t k = 1; k < first.size(); k++) first[k] += first[k - 1];
+        std::vector<uint64_t> at(first.begin(), first.end() - 1);
+        entries.resize(E);
+        for (uint64_t e = 0; e < E; e++) entries[at[ek[e] / VL_VMRANGES]++] = {(uint16_t)(ek[e] % VL_VMRANGES), ec[e]};
+        for (size_t k = 0; k + 1 < first.size(); k++) std::sort(entries.begin() + first[k], entries.begin() + first[k + 1]);
+    };
+    agg.write = [&](const std::vector<uint64_t>& order) {
+        const uint64_t E = entries.size();
+        if (E > cap_entries) throw BadInput("vmrange entries buffer too small (the needed size is reported)");
+        if (!out_entry_offsets || (E && (!out_entry_ranges || !out_entry_hits))) throw BadInput("hits output buffer missing");
+        uint64_t o = 0;
+        out_entry_offsets[0] = 0;
+        for (uint64_t i = 0; i < order.size(); i++)
+            for (uint32_t f = 0; f < nv; f++) {
+                const uint64_t k = order[i] * nv + f;
+                for (uint64_t e = first[k]; e < first[k + 1]; e++, o++) { out_entry_ranges[o] = entries[e].first; out_entry_hits[o] = entries[e].second; }
+                out_entry_offsets[i * nv + f + 1] = o;
+            }
+    };
+    if (out_entry_offsets) out_entry_offsets[0] = 0;
+    return hits_groups(ctx, q, by_buckets, value_names, value_name_lens, nvalues, "vlscan_hits_vmranges", out_buckets, out_counts, cap_groups, out_key_bytes,
+                       cap_key_bytes, out_key_offsets, out_info, 6, &agg);
+}
+int vlscan_vmrange_index(double v) { return vmr_index_host(v); }
+int vlscan_vmrange_text(uint32_t index, char* buf, size_t cap) {
+    if (index >= VL_VMRANGES) return -2;
+    const std::string& t = vmr_texts()[index];
+    if (t.size() > cap) return -1;
+    memcpy(buf, t.data(), t.size());
+    return (int)t.size();
 }
 
 // the limit-th largest of the n int64 keys (weights: NULL = 1 each) into the radix state st (RS_COUNT words + VL_RADIX_PASSES histograms), on

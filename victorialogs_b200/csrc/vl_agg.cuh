@@ -525,6 +525,137 @@ static __global__ void __launch_bounds__(256) k_stats_values(BatchView B, StatsQ
     }
 }
 
+// ---- `stats by (_time:step offset off, f1, ...) histogram(v...)`: per group and value field the numbers counted per vmrange ---------------------
+// (lib/logstorage/stats_histogram.go; metrics.Histogram.Update).  Both reference paths read a cell the same way, so, unlike the sums, nothing
+// depends on whether a block's hits fall in one group.  The index of a number is a binary search over the VL_VMR_BOUNDS boundaries the host
+// computed from its restatement of Go's Log10 (vl_agg.cu, vmr_bounds): no transcendental runs on the device, and the host's
+// vlscan_vmrange_index, the same search, gives the same index by construction.  Counts are exact integers in a table keyed by
+// (g * nv + f) * VL_VMRANGES + index, which grows like the hits table.
+#define VL_VMRANGES 488
+#define VL_VMR_BOUNDS 487   // bound k: the least double whose index is k + 1
+struct VmrTable {
+    unsigned long long* keys;    // [mask + 1]: 0 = empty, else key + 1
+    unsigned long long* cnt;     // [mask + 1]
+    unsigned long long* state;   // [0] slots claimed, [1] overflow, [2] entries compacted, [3] (block, value field) cells on the header fast path
+    uint64_t mask, limit;
+};
+// Histogram.Update's index of x: -1 for NaN and x < 0 (-0 is not below 0 and lands in index 0)
+static __device__ __forceinline__ int vmr_index(const double* bounds, double x) {
+    if (isnan(x) || x < 0) return -1;
+    uint32_t lo = 0, hi = VL_VMR_BOUNDS;
+    while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if (bounds[m] <= x) lo = m + 1; else hi = m; }
+    return (int)lo;
+}
+// add c to `key`; a claim beyond the load limit, or a full table, raises the overflow flag and the host runs the pass again on a larger table
+static __device__ void vmr_add(const VmrTable& M, uint64_t key, uint64_t c) {
+    if (*(volatile unsigned long long*)&M.state[1]) return;
+    uint64_t s = mix64(key) & M.mask;
+    for (uint64_t p = 0; p <= M.mask; p++, s = (s + 1) & M.mask) {
+        unsigned long long cur = *(volatile unsigned long long*)&M.keys[s];
+        if (cur == 0) {
+            cur = atomicCAS(&M.keys[s], 0ull, (unsigned long long)key + 1);
+            if (cur == 0) {
+                if (atomicAdd(&M.state[0], 1ull) >= M.limit) atomicExch(&M.state[1], 1ull);
+                atomicAdd(&M.cnt[s], (unsigned long long)c);
+                return;
+            }
+        }
+        if (cur == key + 1) { atomicAdd(&M.cnt[s], (unsigned long long)c); return; }
+    }
+    atomicExch(&M.state[1], 1ull);
+}
+// One CTA per block with hits (grid-stride), each value field in turn.  Where every row of the cell has one index it is found once: a const
+// cell (one tryParseNumber), or a uint8..uint64 cell / an int64 cell with minimum >= 0 whose header minimum and maximum have one index (the
+// header fast path; float64 stays off it, its NaN rows count nothing).  A dict cell in the plain layout maps its entries once.  Other cells read
+// every hit's number (stats_number's sumValues reading is the histogram's: tryParseNumber, float64(n), the stored double).  A block whose hits
+// are one group then counts its indexes in shared memory and adds one entry per index, else runs of equal (group, index) in each warp add once.
+static __global__ void __launch_bounds__(256) k_stats_vmranges(BatchView B, StatsQuery sq, HitsView V, const uint32_t* __restrict__ hit_slot,
+                                                               const uint32_t* __restrict__ slot_group, const double* __restrict__ bounds, VmrTable M,
+                                                               const uint32_t* __restrict__ counts, const uint64_t* __restrict__ hit_offs, unsigned long long* __restrict__ stats) {
+    __shared__ double s_bounds[VL_VMR_BOUNDS];
+    __shared__ uint32_t s_hist[VL_VMRANGES];
+    __shared__ int s_dict[256], s_one;
+    const int PER_ROW = 0x7FFFFFFF;
+    for (uint32_t i = threadIdx.x; i < VL_VMR_BOUNDS; i += blockDim.x) s_bounds[i] = bounds[i];
+    __syncthreads();
+    for (uint32_t b = blockIdx.x; b < B.nblocks; b += gridDim.x) {
+        const uint32_t n = counts[b];
+        if (n == 0) continue;
+        const uint64_t h0 = hit_offs[b];
+        const uint32_t s0 = hit_slot[h0];
+        bool same = true;
+        for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) same = same && hit_slot[h0 + i] == s0;
+        const bool whole = __syncthreads_and(same);
+        const uint32_t g0 = slot_group[s0];
+        for (uint32_t f = 0; f < sq.nv; f++) {
+            const DevColumn* c = cell_at(B, sq.slot[f], b);
+            if (!c || (c->kind != COL_CONST && c->kind != COL_VALUES)) continue;
+            const uint8_t vt = c->kind == COL_VALUES ? c->vt : VT_STRING;
+            if (vt == VT_IPV4 || vt == VT_ISO8601) continue;
+            const uint8_t* ids = vt == VT_DICT ? plain_dict_ids(B, *c, B.blk_rows[b]) : nullptr;
+            if (threadIdx.x == 0) {
+                int one = PER_ROW;
+                if (c->kind == COL_CONST) {
+                    double x;
+                    one = vl::mn::parse_number(vl::mn::Span{B.hdr + c->meta_off, c->meta_len}, &x) ? vmr_index(s_bounds, x) : -1;
+                } else if (vt == VT_UINT8 || vt == VT_UINT16 || vt == VT_UINT32 || vt == VT_UINT64 || (vt == VT_INT64 && (long long)c->min_value >= 0)) {
+                    const int lo = vmr_index(s_bounds, (double)c->min_value), hi = vmr_index(s_bounds, (double)c->max_value);
+                    if (lo == hi) { one = lo; atomicAdd(&M.state[3], 1ull); }
+                }
+                s_one = one;
+            }
+            if (ids)
+                for (uint32_t k = threadIdx.x; k < c->dict_len; k += blockDim.x) {
+                    const uint32_t* dof = (const uint32_t*)(B.hdr + c->meta_off);
+                    double x;
+                    s_dict[k] = vl::mn::parse_number(vl::mn::Span{B.hdr + c->meta_off + 4 * (c->dict_len + 1) + dof[k], dof[k + 1] - dof[k]}, &x) ? vmr_index(s_bounds, x) : -1;
+                }
+            __syncthreads();
+            const int one = s_one;
+            auto index_at = [&](uint32_t r) -> int {
+                if (one != PER_ROW) return one;
+                if (ids) {
+                    if (ids[r] < c->dict_len) return s_dict[ids[r]];
+                    atomicMax(&stats[ST_ERROR], (unsigned long long)ERR_DICT_INDEX);
+                    return -1;
+                }
+                double x; bool has;
+                stats_number(B, c, b, r, sq.row_off8[f], true, &x, &has, stats);
+                return has ? vmr_index(s_bounds, x) : -1;
+            };
+            auto key = [&](uint32_t g, int x) { return ((uint64_t)g * sq.nv + f) * VL_VMRANGES + (uint32_t)x; };
+            if (whole && one != PER_ROW) {
+                if (threadIdx.x == 0 && one >= 0) vmr_add(M, key(g0, one), n);
+            } else if (whole) {
+                for (uint32_t k = threadIdx.x; k < VL_VMRANGES; k += blockDim.x) s_hist[k] = 0;
+                __syncthreads();
+                for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) { const int x = index_at(V.hits[h0 + i]); if (x >= 0) atomicAdd(&s_hist[x], 1u); }
+                __syncthreads();
+                for (uint32_t k = threadIdx.x; k < VL_VMRANGES; k += blockDim.x) if (s_hist[k]) vmr_add(M, key(g0, (int)k), s_hist[k]);
+            } else {
+                for (uint32_t base = 0; base < n; base += blockDim.x) {
+                    const uint32_t i = base + threadIdx.x;
+                    const bool valid = i < n;
+                    const uint32_t g = valid ? slot_group[hit_slot[h0 + i]] : 0;
+                    const int x = valid ? index_at(V.hits[h0 + i]) : -1;
+                    const uint32_t run = warp_run_end(x >= 0, true, g, (uint32_t)x);
+                    if (run) vmr_add(M, key(g, x), run);
+                }
+            }
+            __syncthreads();   // s_one, s_dict and s_hist are rewritten for the next field
+        }
+    }
+}
+// the occupied slots of the vmrange table -> (key, count) entries, in no particular order (the host sorts them)
+static __global__ void k_vmr_compact(VmrTable M, unsigned long long* __restrict__ out_keys, unsigned long long* __restrict__ out_cnt) {
+    const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s > M.mask) return;
+    const unsigned long long k = M.keys[s];
+    if (!k) return;
+    const uint64_t e = atomicAdd(&M.state[2], 1ull);
+    out_keys[e] = k - 1; out_cnt[e] = M.cnt[s];
+}
+
 // ---- the N newest selected rows: `/select/logsql/query?limit=N` (app/vlselect/logsql/logsql.go:1005-1080 getLastNQueryResults) ----------------
 // Timestamps inside a block never decrease (the writer refuses anything else, lib/logstorage/block.go:182,346), so every selected row of block b
 // lies in [min_b, max_b] of its header.  A weighted radix select over the minimums of the blocks with hits at or above the floor (weight: their

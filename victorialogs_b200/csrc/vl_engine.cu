@@ -760,7 +760,7 @@ void vlscan_ctx_free(vlscan_ctx* ctx) {
     for (auto& r : ctx->row_off8) r.release();
     for (auto& r : ctx->ready) r.release();
     ctx->zsrc.release(); ctx->zcols.release(); ctx->ztest.release(); ctx->ts_vals.release();
-    for (DevBuf* b : {&ctx->hit_block, &ctx->glens, &ctx->goffs, &ctx->gtiles, &ctx->gout, &ctx->gstat, &ctx->hslot, &ctx->hblk, &ctx->htab, &ctx->hgrp, &ctx->lcand, &ctx->ftab, &ctx->patch, &ctx->unstaged}) b->release();
+    for (DevBuf* b : {&ctx->hit_block, &ctx->glens, &ctx->goffs, &ctx->gtiles, &ctx->gout, &ctx->gstat, &ctx->hslot, &ctx->vagg, &ctx->hblk, &ctx->htab, &ctx->hgrp, &ctx->lcand, &ctx->ftab, &ctx->patch, &ctx->unstaged}) b->release();
     for (DevBuf& b : ctx->ftxt) b.release();
     zstd_dev_free(ctx->zdev);
     delete ctx->pool;

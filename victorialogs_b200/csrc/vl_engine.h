@@ -122,7 +122,8 @@ struct vlscan_ctx {
     vl::DevBuf hit_block, glens, goffs, gtiles, gout, gstat;   // build_hit_list: block of each hit; text_offsets / text_bytes (vlscan_gather_values,
                                            // hits, last rows, facets): value lengths / offsets, exclusive_scan's tile sums, output staging; the error slot
     vl::DevBuf ts_vals;                    // decoded timestamps / running sums, 8 bytes per row of the batch (k_time_match, decode_listed_timestamps)
-    vl::DevBuf hslot;                      // vlscan_hits_sums: the group-table slot of every hit (k_hits_group<true>)
+    vl::DevBuf hslot;                      // vlscan_hits_sums / _vmranges: the group-table slot of every hit (k_hits_group<true>)
+    vl::DevBuf vagg;                       // vlscan_hits_vmranges: the boundaries, the vmrange table and its compacted entries, laid out by Carve
     vl::DevBuf hblk, htab, hgrp;           // laid out by Carve.  vlscan_hits_stats: per-block bucket + multi-bucket flag, the group table (tags,
                                            // counts, state), the emitted groups.  vlscan_last_rows: per-block keys / candidate offsets / weights /
                                            // counts / marks and the candidate and decode lists, the radix select states, the chosen rows.

@@ -108,7 +108,7 @@ EXPORTS = ["vlscan_device_count", "vlscan_ctx_create", "vlscan_ctx_free", "vlsca
            "vlscan_batch_upload", "vlscan_batch_free", "vlscan_batch_nblocks", "vlscan_batch_rows", "vlscan_batch_words", "vlscan_batch_device_bytes",
            "vlscan_batch_generate", "vlscan_batch_download", "vlscan_host_blocks_get", "vlscan_host_blocks_field", "vlscan_host_blocks_bytes",
            "vlscan_host_blocks_free", "vlscan_host_blocks_compress", "vlscan_zstd_decompress", "vlscan_zstd_inspect", "vlscan_zstd_walk_digest", "vlscan_part_open", "vlscan_part_free", "vlscan_part_header", "vlscan_part_nblocks", "vlscan_part_block_header", "vlscan_part_timestamps",
-           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_hits_sums", "vlscan_hits_stats_bucketed", "vlscan_hits_sums_bucketed", "vlscan_truncate_timestamp", "vlscan_bucket_text", "vlscan_last_rows", "vlscan_facets", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch",
+           "vlscan_part_ncolumn_names", "vlscan_part_column_name", "vlscan_part_blocks", "vlscan_host_blocks_source", "vlscan_scan_resident", "vlscan_last_scan_stats", "vlscan_fetch_results", "vlscan_fetch_hits", "vlscan_gather_timestamps", "vlscan_gather_values", "vlscan_hits_stats", "vlscan_hits_sums", "vlscan_hits_stats_bucketed", "vlscan_hits_sums_bucketed", "vlscan_hits_vmranges", "vlscan_vmrange_index", "vlscan_vmrange_text", "vlscan_truncate_timestamp", "vlscan_bucket_text", "vlscan_last_rows", "vlscan_facets", "vlscan_result_digest", "vlscan_totals_sum", "vlscan_result_device_ptrs", "vlscan_scan_batch",
            "vlscan_scan_batch_keep", "vlscan_stage_selected"]
 
 
@@ -140,6 +140,8 @@ def lib():
             getattr(L, n).restype = None
         L.vlscan_truncate_timestamp.argtypes = [C.c_int64, C.c_int64, C.c_int64, C.c_uint32]
         L.vlscan_truncate_timestamp.restype = C.c_int64
+        L.vlscan_vmrange_index.argtypes = [C.c_double]
+        L.vlscan_vmrange_text.argtypes = [C.c_uint32, C.c_char_p, C.c_size_t]
         L.vlscan_format_float64.argtypes = [C.c_uint64, C.c_char_p, C.c_size_t]
         L.vlscan_format_float64.restype = C.c_int
         _LIB = L
@@ -303,6 +305,40 @@ def stats_merge(states):
                 continue
             r0, v0 = out[k]
             out[k] = (r0 + rows, [(b if math.isnan(a) else a if math.isnan(b) else a + b, ca + cb) for (a, ca), (b, cb) in zip(v0, vals)])
+    return out
+
+
+VMRANGES = 488   # VLSCAN_VMRANGES: vmrange indexes 0 (lower) .. 487 (upper), in numeric order
+
+
+def vmrange_index(v):
+    """The vmrange index of one number as Histogram.Update files it (vlscan_vmrange_index: host build of the kernel's mapping); -1 for NaN
+    and negative numbers, which it skips"""
+    return lib().vlscan_vmrange_index(float(v))
+
+
+def vmrange_text(index):
+    """The vmrange text of index 0 .. VMRANGES - 1 ("0...1.000e-09", "1.000e-09...1.136e-09", ..., "1.000e+18...+Inf")"""
+    out = C.create_string_buffer(64)
+    n = lib().vlscan_vmrange_text(index, out, 64)
+    if n < 0:
+        raise ValueError(index)
+    return out.raw[:n].decode()
+
+
+def vmranges_merge(states):
+    """The merge a caller runs over the per-batch states of Ctx.hits_vmranges (pipeStatsGroup.mergeState with
+    statsHistogramProcessor.mergeState, lib/logstorage/stats_histogram.go) -> {(bucket, key texts): (rows, [{index: hits} per value field])}.
+    Rows add, and so do the hits of each (value field, index)."""
+    out = {}
+    for st in states:
+        for bucket, keys, rows, vals in st:
+            k = (bucket, keys)
+            r0, v0 = out.get(k, (0, [{} for _ in vals]))
+            for m, add in zip(v0, vals):
+                for i, h in add.items():
+                    m[i] = m.get(i, 0) + h
+            out[k] = (r0 + rows, v0)
     return out
 
 
@@ -954,6 +990,47 @@ class Ctx:
         G = int(out_info[0])
         keys = _row_texts(kb.tobytes(), offs, G, nby)
         return [(int(buckets[g]), keys[g], int(counts[g]), [(float(sums[g * nv + f]), int(vcounts[g * nv + f])) for f in range(nv)]) for g in range(G)]
+
+    def hits_vmranges(self, step, offset=0, calendar=BUCKET_PLAIN, by=(), values=(), batch=None, info=None, buckets=None):
+        """`stats by (_time:step offset off, by...) histogram(v)...` over the selected rows of the last scan (vlscan_hits_vmranges)
+        -> [(bucket, (key texts as bytes...), rows, [{vmrange index: hits} per value field])] in the order of hits_stats; vmrange_text names
+        an index.  `info` (a dict) receives what hits_stats gives, plus entries and header_cells (cells counted from their header alone);
+        buckets as for hits_stats."""
+        batch = batch or getattr(self, "_last", None)
+        q, keep = hits_query(step, offset, calendar, by)
+        bks = by_buckets(buckets, len(by))
+        vn = [_b(f) for f in values]
+        varr = (C.c_char_p * max(len(vn), 1))(*vn)
+        vlens = (C.c_size_t * max(len(vn), 1))(*[len(x) for x in vn])
+        nby, nv = len(by), len(vn)
+        out_info = (C.c_uint64 * 6)()
+
+        def call(cap_groups, cap_bytes, cap_entries):
+            buckets = np.zeros(cap_groups, dtype=np.int64)
+            counts = np.zeros(cap_groups, dtype=np.uint64)
+            offs = np.zeros(cap_groups * nby + 1, dtype=np.uint64)
+            kb = np.zeros(max(cap_bytes, 1), dtype=np.uint8)
+            eoffs = np.zeros(cap_groups * nv + 1, dtype=np.uint64)
+            ranges = np.zeros(max(cap_entries, 1), dtype=np.uint16)
+            hits = np.zeros(max(cap_entries, 1), dtype=np.uint64)
+            rc = lib().vlscan_hits_vmranges(self.h, C.byref(q), bks, varr, vlens, C.c_uint32(nv), buckets.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p),
+                                            C.c_uint64(cap_groups), kb.ctypes.data_as(C.c_void_p), C.c_uint64(cap_bytes), offs.ctypes.data_as(C.c_void_p),
+                                            eoffs.ctypes.data_as(C.c_void_p), ranges.ctypes.data_as(C.c_void_p), hits.ctypes.data_as(C.c_void_p), C.c_uint64(cap_entries), out_info)
+            return rc, (buckets, counts, offs, kb, eoffs, ranges, hits)
+        cap = max(1, min(int(batch.rows) if batch else 0, 1 << 16))
+        buckets, counts, offs, kb, eoffs, ranges, hits = self._call_grown(call, (cap, 1 << 16, cap * max(nv, 1)), lambda: (out_info[0], out_info[1], out_info[4]))
+        if info is not None:
+            info.update(groups=out_info[0], key_bytes=out_info[1], rows=out_info[2], blocks_decoded=out_info[3], entries=out_info[4], header_cells=out_info[5])
+        G = int(out_info[0])
+        keys = _row_texts(kb.tobytes(), offs, G, nby)
+        out = []
+        for g in range(G):
+            vals = []
+            for f in range(nv):
+                a, z = int(eoffs[g * nv + f]), int(eoffs[g * nv + f + 1])
+                vals.append({int(ranges[e]): int(hits[e]) for e in range(a, z)})
+            out.append((int(buckets[g]), keys[g], int(counts[g]), vals))
+        return out
 
     def last_rows(self, limit, fields=(), min_timestamp=None, info=None):
         """The `limit` newest selected rows of the last scan with _time >= min_timestamp (vlscan_last_rows)
